@@ -1,14 +1,18 @@
-"""bench.py — images/sec of the G+D training cycle (BASELINE.json metric) on N B200s of one node.
+"""bench.py — images/sec of the G+D training cycle (BASELINE.json metric) on N H100s of one node.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload resnet_cifar10]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload resnet_cifar10] [--dump-outputs DIR]
 
 A "step" is one ModularGAN cycle of `resnet_cifar10.gin` at batch 256 per GPU: disc_iters=5 D-updates +
 1 G-update on fresh synthetic images/z (unrolled semantics, reference gans/modular_gan.py:218-223), i.e.
 256*6 images consumed per GPU per step.  Prints ONE JSON line (rank 0).  The line also carries, under "workloads", the
-other half of BASELINE's metric — `biggan_imagenet128` at 256 images per GPU (config C5's per-GPU share) — and at
+other half of BASELINE's metric — `biggan_imagenet128` at 64 images per GPU (80 GB does not hold C5's 256) — and at
 `--gpus 4` BASELINE config C4 (`resnet_lsun-bedroom128`, WGAN-GP, 64 per GPU), each with its own step time and
 useful-FLOP fraction; "eval" is FID samples/sec; "fp32_step" the same cifar cycle in math_mode 0; at N > 1
 "dp_equivalence" is an in-run check that N ranks on shards reproduce one rank on the concatenated batch.
+
+--dump-outputs DIR writes what the last timed step computed (losses, and the parameters and gradients of G and D after
+it; a fixed seeded sample of vectors above DUMP_MAX_ELEMS) as DIR/<name>.npy.  The cycle's inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -29,7 +33,9 @@ WORKLOADS = {
     "resnet_cifar10": dict(batch=256, gflop_per_slot_image=39.05, eval_samples=2048),
     "sndcgan_celebahq128": dict(batch=128, gflop_per_slot_image=78.95, eval_samples=512),
     "resnet_lsun-bedroom128": dict(batch=64, gflop_per_slot_image=559.2, eval_samples=512),
-    "biggan_imagenet128": dict(batch=256, gflop_per_slot_image=434.4, eval_samples=512),
+    # BigGAN-128 at 64 images per GPU (a global batch of 2048 over 32 GPUs): 256 per GPU, BASELINE C5's share of 8 GPUs,
+    # needs more than the 80 GB of an H100
+    "biggan_imagenet128": dict(batch=64, gflop_per_slot_image=434.4, eval_samples=512),
 }
 
 
@@ -50,11 +56,12 @@ def peaks():
     d = json.load(open(p))
     return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained"),
             "source": "measured"}
-  return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+  # NVIDIA H100 SXM data sheet (700 W card), dense BF16: a bound, not a measured rate
+  return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler(object):
-  """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks / throttle reasons sampled (read only) DURING the timed region."""
 
   def __init__(self, index):
     self.index, self.rows, self.proc = index, [], None
@@ -114,7 +121,7 @@ def build_engine(workload, batch, seed=0, math_mode=1):
 def time_dominant_kernel(b, iters=20, math_mode=1):
   """Roofline evidence for the dominant kernel: the 3x3 256->256 conv of G's B3 block at 32x32 (conv2), batch = bench batch
   (SURVEY App. B: 1208 MF/img), timed alone with CUDA events on the launching stream; its 268 MB input and
-  268 MB output exceed the 126 MB L2, so every launch streams from HBM.  In the training step this convolution reads the
+  268 MB output exceed the 50 MB L2 of an H100, so every launch streams from HBM.  In the training step this convolution reads the
   output of the fused BN+ReLU kernel, which is stored TF32-rounded: `ms` times that variant (operand already rounded, no
   in-kernel rounding pass); `ms_inkernel_rounding` the variant that rounds an arbitrary fp32 operand in shared memory."""
   import torch
@@ -140,7 +147,7 @@ def time_dominant_kernel(b, iters=20, math_mode=1):
   x.tf32 = False
   ms_round = timed()
   flops = 2.0 * b * 32 * 32 * 256 * 256 * 9
-  name = "conv_tc_kernel (tcgen05 kind::tf32 + weight prep)" if math_mode == 1 else "gather_gemm_kernel<FWD> (fp32 SIMT)"
+  name = "conv_tc_kernel (wgmma tf32 + weight prep)" if math_mode == 1 else "gather_gemm_kernel<FWD> (fp32 SIMT)"
   return {"kernel": "%s conv3x3 256->256 @32x32 B=%d" % (name, b), "ms": ms, "tflops": flops / ms / 1e9,
           "ms_inkernel_rounding": ms_round, "flops_per_launch": flops}
 
@@ -222,6 +229,23 @@ def measure_cycle(workload, b, steps, warmup, mm, world, rank, eager=False, e2e=
   d_losses, g_loss = eng.read_losses()
   return {"eng": eng, "ds": ds, "options": options, "k": k, "ms_dev": ms_dev, "ms_e2e": ms_e2e, "h2d_bytes": h2d_bytes,
           "launches_per_cycle": launches_per_cycle, "graph": graph, "losses": {"d": d_losses, "g": g_loss}}
+
+
+DUMP_MAX_ELEMS = 15 << 18          # per array (15 MB of float32): four parameter / gradient vectors stay below 64 MB
+
+
+def dump_outputs(eng, out_dir):
+  """Writes the results of the engine's last cycle as out_dir/<name>.npy (float64 losses, float32 vectors)."""
+  os.makedirs(out_dir, exist_ok=True)
+  d_losses, g_loss = eng.read_losses()
+  np.save(os.path.join(out_dir, "d_losses.npy"), np.asarray(d_losses, np.float64))
+  np.save(os.path.join(out_dir, "g_loss.npy"), np.asarray([g_loss], np.float64))
+  for net, flat in (("g", eng.flat_g), ("d", eng.flat_d)):
+    for kind in ("param", "grad"):
+      a = flat[kind].t.detach().float().cpu().numpy().ravel()
+      if a.size > DUMP_MAX_ELEMS:        # the same seeded sample of elements in every run
+        a = a[np.sort(np.random.RandomState(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))]
+      np.save(os.path.join(out_dir, "%s_%s.npy" % (net, kind)), a.astype(np.float32))
 
 
 def release(m):
@@ -324,6 +348,8 @@ def run_ours(args):
   m = measure_cycle(args.workload, b, args.steps, args.warmup, mm, world, rank, eager=args.eager, prof=prof)
   clocks = sampler.stop() if rank == 0 else None
   eng, ds, options, k = m["eng"], m["ds"], m["options"], m["k"]
+  if args.dump_outputs and rank == 0:
+    dump_outputs(eng, args.dump_outputs)
   ms_dev, ms_e2e = m["ms_dev"], m["ms_e2e"]
   images_per_step = b * (k + 1) * world
   value = images_per_step * args.steps / (ms_dev / 1e3)
@@ -345,7 +371,7 @@ def run_ours(args):
     sub_steps = max(3, min(args.steps, 5))
     names = []
     if args.workload == "resnet_cifar10":
-      names.append("biggan_imagenet128")                       # the other half of BASELINE's metric (C5's per-GPU share)
+      names.append("biggan_imagenet128")                       # the other half of BASELINE's metric (C5's workload)
       if world == 4:
         names.append("resnet_lsun-bedroom128")                 # BASELINE config C4: WGAN-GP, 256 over 4 GPUs
     for name in names:
@@ -378,8 +404,8 @@ def run_ours(args):
         "dtype": "tf32" if mm else "f32", "data": "synthetic",
         "config": {"workload": config_workload,
                    "global_batch": b * world, "parallelism": "dp%d" % world, "cuda_graph": m["graph"],
-                   "l2": "activations per cycle (GBs) exceed the 126 MB L2: inputs larger than L2",
-                   "math_mode": ("1: tcgen05 kind::tf32 convolutions (operands rounded to nearest TF32, fp32 TMEM accumulate) "
+                   "l2": "activations per cycle (GBs) exceed the 50 MB L2: inputs larger than L2",
+                   "math_mode": ("1: wgmma tf32 convolutions (operands rounded to nearest TF32, fp32 accumulate) "
                                  "where the shape allows, fp32 elsewhere") if mm else "0: fp32 SIMT contraction"},
         "e2e": {"value": e2e_value, "unit": "images/sec", "h2d_bytes_per_step": m["h2d_bytes"],
                 "d2h_bytes_per_step": 4 * (k + 1), "ms_per_step": ms_e2e / args.steps},
@@ -390,8 +416,8 @@ def run_ours(args):
                      "frac_of_tf32_peak": dom["tflops"] / (pk["bf16_tflops"] / 2.0),
                      "traffic": traffic, "traffic_source": traffic_src,
                      "kernel": dom["kernel"], "kernel_ms": dom["ms"], "kernel_ms_inkernel_rounding": dom["ms_inkernel_rounding"],
-                     "peak_kind": "%s dense bf16 cuBLAS burst (MEASURED_PEAKS.json); the kernel computes in TF32, whose tensor "
-                                  "peak is nominally half of it (frac_of_tf32_peak)" % pk["source"],
+                     "peak_kind": "dense bf16 peak (%s); the kernel computes in TF32, whose tensor peak is nominally half "
+                                  "of it (frac_of_tf32_peak)" % pk["source"],
                      "step_useful_tflops_per_gpu": cyc_tflop / (ms_dev / args.steps / 1e3),
                      "step_frac": cyc_tflop / (ms_dev / args.steps / 1e3) / (pk["bf16_tflops_sustained"] or pk["bf16_tflops"])},
         "cpu_baseline": cpu,
@@ -540,6 +566,8 @@ def main():
   ap.add_argument("--dp-check", action="store_true", help="with --headline-only at N > 1: still run the in-run dp_equivalence check")
   ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU oracle leg (profiling runs only)")
   ap.add_argument("--eager", action="store_true", help="do not capture the cycle into a CUDA graph (profiling runs only)")
+  ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                  help="write the losses, parameters and gradients of the last timed step as DIR/<name>.npy")
   args = ap.parse_args()
   if args.impl == "reference":
     run_reference(args)

@@ -1,5 +1,5 @@
 """Ops library: same names, arguments and error behaviour as the reference's
-compare_gan/architectures/arch_ops.py, with every computation dispatched to sm_100a kernels
+compare_gan/architectures/arch_ops.py, with every computation dispatched to sm_90a kernels
 through the C-ABI (kernels.py).  Inputs/outputs are device tensors (tape.DT), NHWC float32.
 """
 import functools
@@ -110,7 +110,7 @@ def standardize_batch(inputs, is_training, decay=0.999, epsilon=1e-3, data_forma
   if data_format not in {"NCHW", "NHWC"}:
     raise ValueError("Invalid data_format {}. Allowed: NCHW, NHWC.".format(data_format))
   if data_format != "NHWC":
-    raise ValueError("Only NHWC is implemented on the B200 path.")
+    raise ValueError("Only NHWC is implemented on the H100 path.")
   if use_cross_replica_mean is None:
     use_cross_replica_mean = tpu_ops.num_replicas() > 1
   rank = len(inputs.shape)

@@ -1,7 +1,7 @@
 """BigGAN networks for 32..512 pixels (reference architectures/resnet_biggan.py:80-425; Brock et al. 2018) as tables:
 a channel plan per resolution, one residual-block family (1x1 shortcut, evaluated last, dropped in the discriminator
 when the widths agree), the non-local block after the named blocks, hierarchical z + class embedding feeding every
-conditional batch norm, projection discriminator.  All convolutions / matmuls dispatch to the tcgen05 kernels through
+conditional batch norm, projection discriminator.  All convolutions / matmuls dispatch to the tensor-core kernels through
 `arch_ops`."""
 from .. import gin_lite as gin
 from .. import kernels as K

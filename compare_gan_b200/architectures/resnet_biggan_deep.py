@@ -96,7 +96,7 @@ class Generator(abstract_arch.AbstractGenerator):
   def __init__(self, ch=128, embed_y=True, embed_y_dim=128, experimental_fast_conv_to_rgb=False, **kwargs):
     super(Generator, self).__init__(**kwargs)
     if experimental_fast_conv_to_rgb:
-      raise NotImplementedError("experimental_fast_conv_to_rgb is a TPU layout trick; the final conv is a thin tcgen05 tile here")
+      raise NotImplementedError("experimental_fast_conv_to_rgb is a TPU layout trick; the final conv is a thin tensor-core tile here")
     self._ch, self._embed_y, self._embed_y_dim = ch, embed_y, embed_y_dim
 
   def _resnet_block(self, name, in_channels, out_channels, scale):

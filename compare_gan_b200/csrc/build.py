@@ -1,4 +1,4 @@
-"""Build libcgan_b200.so in-tree with nvcc for sm_100a (no torch headers, plain C-ABI)."""
+"""Build libcgan_b200.so in-tree with nvcc for sm_90a (no torch headers, plain C-ABI)."""
 import glob
 import os
 import subprocess
@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "libcgan_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default", "-Wno-deprecated-gpu-targets"]
 
 

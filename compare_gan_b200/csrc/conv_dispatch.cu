@@ -1,4 +1,4 @@
-// Public conv entry points: choose between the exact-fp32 gather-GEMM (gemm.cu, math_mode 0) and the tcgen05
+// Public conv entry points: choose between the exact-fp32 gather-GEMM (gemm.cu, math_mode 0) and the wgmma
 // tensor-core implicit GEMM (conv_tc.cu, math_mode 1) according to the context's math mode and the shape.
 #include "common.cuh"
 
@@ -91,7 +91,7 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   const bool x_tf32 = ep && (ep->flags & CGAN_CONV_IN_TF32);
   CGAN_REQUIRE(ctx, ldy >= d->cout, "ldy must be >= cout");
   CGAN_REQUIRE(ctx, ldy == d->cout || !d->upsample, "strided output is not available with upsample");
-  const bool ld_ok = ldy == d->cout || ldy % 4 == 0;      // the tcgen05 epilogue stores float4
+  const bool ld_ok = ldy == d->cout || ldy % 4 == 0;      // the tensor-core epilogue stores rows of float2 pairs (a multiple of 4 keeps them aligned)
   const bool ptr_ok = al16p(x) && al16p(y) && (!bias || al16p(bias)) && (!ep || ((!ep->residual || al16p(ep->residual)) &&
                                                                                   (!ep->mask || al16p(ep->mask))));
   TcExtra ex = tc_extra(ep, x_tf32);

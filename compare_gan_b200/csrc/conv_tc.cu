@@ -1,20 +1,20 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM convolution for sm_100a — math_mode 1.
+// Warpgroup-MMA (wgmma, sm_90a) implicit-GEMM convolution — math_mode 1.
 //
 //   out[pixel, co] = sum_{tap, ci} in[pixel + off(tap), ci] * wt[tap][co][ci]        (+ bias[co])
 //
 // * A operand (activations, NHWC fp32): one TMA 4-D tiled load per (tap, 32-channel chunk) brings a
 //   [images x rows x cols x 32ch] box = 128 pixels x 128 B straight into the 128B-swizzled K-major layout
-//   the UMMA descriptor expects; TF SAME padding is the TMA out-of-bounds zero fill (negative coordinates),
+//   the wgmma descriptor expects; TF SAME padding is the TMA out-of-bounds zero fill (negative coordinates),
 //   so no im2col buffer and no padding pass exist.
 // * B operand (weights): pre-rounded (round-to-nearest TF32) and laid out [tap][row][k] K-major by a small
 //   prep kernel; TMA 3-D loads.
-// * The fp32 activations are rounded to nearest TF32 IN SHARED MEMORY by the (otherwise idle) epilogue
-//   warps before the tensor core reads them — tcgen05 kind::tf32 would otherwise truncate the low 13 bits,
-//   a systematic -2^-11 relative bias per product that accumulates through a 13-layer discriminator.
-// * D accumulates in TMEM (128 lanes x N fp32 columns); one elected thread issues tcgen05.mma
-//   (M=128, N<=256, K=8 per instruction); completion is tracked with tcgen05.commit -> mbarrier.
-// * Warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..5 = operand
-//   rounding during the main loop, then epilogue (tcgen05.ld -> +bias -> global).
+// * The fp32 activations are rounded to nearest TF32 IN SHARED MEMORY by the consumer warpgroups before their
+//   MMAs read them — the tensor core would otherwise truncate the low 13 bits, a systematic -2^-11 relative bias per
+//   product that accumulates through a 13-layer discriminator.
+// * Warp roles: warps 0..7 = two consumer warpgroups, warpgroup g owning rows 64g..64g+63 of every 128-pixel tile:
+//   (operand rounding,) wgmma m64nBNk8 (K = 8 per instruction, fp32 accumulators in registers), epilogue straight from
+//   the accumulator fragments (+bias, residual, ReLU / mask, TF32 rounding -> global); warp 8 = TMA producer.
+//   Stages are released one k-block late (wgmma.wait_group 1), so the rounding of the next stage overlaps the MMAs.
 //
 // The same kernel serves forward and input-gradient convolutions (and the four sub-pixel phases of a
 // conv over a zero-inserted 2x upsampled input): the host supplies, per tap, the input offset and the weight
@@ -25,13 +25,15 @@ namespace {
 
 using namespace tc;
 
-constexpr int TC_BM = 128;          // output pixels per CTA tile (UMMA M)
+constexpr int TC_BM = 128;          // output pixels per CTA tile (two warpgroups x wgmma M = 64)
 constexpr int TC_BK = 32;           // fp32 channels per k-block: 128 B = one swizzle row
-constexpr int TC_MAX_STAGES = 4;   // the pipeline depth is chosen per launch so that TWO CTAs fit an SM (see host code)
+constexpr int TC_MAX_STAGES = 4;
 constexpr int TC_MAX_TAPS = 32;
-constexpr int TC_RWARPS = 8;         // warps 2..9: operand rounding, then the epilogue (two warps per TMEM lane quarter)
-constexpr int TC_THREADS = 64 + 32 * TC_RWARPS;
+constexpr int TC_CWARPS = 8;        // consumer warps (two warpgroups)
+constexpr int TC_THREADS = 32 * TC_CWARPS + 32;     // + the TMA producer warp
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 4;     // 16 KB
+constexpr int TC_WG_A_BYTES = TC_A_BYTES / 2;      // one warpgroup's 64 rows
+constexpr int TC_ACC_COLS = 256;    // mt x bn accumulator columns per CTA: mt*bn/2 registers per consumer thread
 
 struct TcParams {
   int ntaps, kchunks;               // k-blocks = ntaps * kchunks
@@ -41,49 +43,35 @@ struct TcParams {
   int rows_used;                    // bw*bh*bni <= 128 pixel rows actually filled by the TMA box
   int img_n, img_h, img_w;          // extent of the pixel grid (tiles at the border hang over; those rows are not stored)
   int relu;                         // fused ReLU in the epilogue
-  int epi_stage;                    // 1: the epilogue transposes through shared memory for coalesced stores (tc_epilogue)
+  int vec2;                         // 1: every output row starts at an even element offset and cout is even (float2 stores)
   int round_a;                      // 1: round the activation tiles to nearest TF32 in shared memory (operand not pre-rounded)
   int round_out;                    // 1: store TF32-rounded outputs (the consumer is another tensor-core contraction)
   float mask_leak;                  // with `mask`: out = ref > 0 ? v : mask_leak * v  ((leaky-)ReLU backward fused into a dgrad)
   const float* residual;            // optional tensor of the output's geometry added before the activation (residual blocks)
   const float* mask;                // optional tensor of the output's geometry: the (leaky-)ReLU input/output whose sign gates v
   int wimg_stride;                  // batched GEMM: weight slice = wtap + image * wimg_stride (tiles never span images)
-  int bn;                           // UMMA N (multiple of 32, <= 256)
+  int bn;                           // wgmma N (multiple of 32, <= 256)
   int stages;                       // smem pipeline depth (2..4)
-  int mt;                           // pixel tiles per CTA sharing one weight tile (accumulators mt x bn TMEM columns)
+  int mt;                           // pixel tiles per CTA sharing one weight tile (mt x bn accumulator columns)
   int tiles_total;                  // tiles_w * tiles_h * tiles_n
-  int tmem_cols;                    // power of two >= bn
   int cout;                         // valid output channels (row length of `out` pixels)
   long long s_n, s_h, s_w, base;    // output element strides / offset (floats)
   float* out;
   const float* bias;
-  // halo mode (conv_tc_halo_kernel): the taps come in `hg` groups of `hnv` vertically consecutive taps that share their
-  // horizontal offset; one TMA box of bh + hnv - 1 rows serves all taps of a group (the vertical shift is a descriptor
-  // offset of bw rows), so the activation operand crosses L2 -> smem `hg` times per channel chunk instead of hg * hnv
   // sub-pixel phases merged into one launch (blockIdx.z): phase ph owns the taps [ph_tap0[ph], ph_tap0[ph+1]) and writes
   // at element offset ph_base[ph] (a convolution over a zero-inserted input, a stride-2 input gradient)
   int nphases;
   int ph_tap0[5];
   long long ph_base[4];
+  // halo mode (conv_tc_halo_kernel): the taps come in `hg` groups of `hnv` vertically consecutive taps that share their
+  // horizontal offset; one TMA box of bh + hnv - 1 rows serves all taps of a group (the vertical shift is a descriptor
+  // offset of bw rows), so the activation operand crosses L2 -> smem `hg` times per channel chunk instead of hg * hnv
   int hg, hnv;
   int h_off_w[4], h_off_h0[4], h_wtap[4][4];
   int a_halo_bytes;                 // smem footprint of one tile's halo box (1024-aligned)
   int a_box_bytes;                  // bytes TMA writes per halo box
   int sa_stages, sb_stages;
 };
-
-// K-major, 128B-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm100):
-// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major, 1) | SBO>>4 [32,46) = 1024 B between 8-row groups
-// | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
 
 // up to four views of the input tensor (the sub-pixel phases of a 2x-upsampled gradient); plain convs use view 0
 struct AMaps { CUtensorMap m[4]; };
@@ -96,163 +84,109 @@ __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int t, int& ow
   ow0 = tw * p.bw; oh0 = th * p.bh; n0 = tn * p.bni;
 }
 
-// Epilogue of warps 2..9: tcgen05.ld the accumulators of this CTA's tiles, apply bias / residual / ReLU / mask / TF32
-// rounding, store.  TMEM lane quarter is fixed by (warp id % 4); row of the tile = TMEM lane.
-//
-// tcgen05.ld hands every thread 32 consecutive columns of ITS row; storing them from there costs one 16-byte piece in
-// each of 32 different 128-byte lines per instruction — 32 LSU wavefronts, and the epilogue (a fifth of the kernel at
-// one CTA per SM, ncu r2: 129 k wavefronts per SM) is bound by exactly that.  Each warp therefore transposes its
-// 32 x 32 chunk through a private 32 x 36-float staging area in the (by now idle) operand ring, after which a quarter
-// warp owns one row's 128 contiguous bytes: 4 wavefronts per store instruction, and the fused residual / mask reads
-// coalesce the same way.  `stg` = shared address of this warp's staging area (0: none, per-thread rows).
-constexpr int TC_EPI_ROW_BYTES = 36 * 4;                     // 32 columns + 16 B pad: 16-byte aligned, conflict-free v4 access
-constexpr int TC_EPI_WARP_BYTES = 32 * TC_EPI_ROW_BYTES;     // 4608 B per warp, 36 KB per CTA
-
-__device__ __forceinline__ float4 tc_epilogue_math(const TcParams& p, float4 v, const float4 bv, long long off) {
-  v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-  if (p.residual) {
-    const float4 rv = *reinterpret_cast<const float4*>(p.residual + off);
-    v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-  }
-  if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-  if (p.mask) {
-    const float4 mv = *reinterpret_cast<const float4*>(p.mask + off);
-    v.x = mv.x > 0.f ? v.x : p.mask_leak * v.x; v.y = mv.y > 0.f ? v.y : p.mask_leak * v.y;
-    v.z = mv.z > 0.f ? v.z : p.mask_leak * v.z; v.w = mv.w > 0.f ? v.w : p.mask_leak * v.w;
-  }
-  if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w); }
+__device__ __forceinline__ float tc_epilogue_one(const TcParams& p, float v, int col, long long off) {
+  if (p.bias) v += p.bias[col];
+  if (p.residual) v += p.residual[off];
+  if (p.relu) v = fmaxf(v, 0.f);
+  if (p.mask) v = p.mask[off] > 0.f ? v : p.mask_leak * v;
+  if (p.round_out) v = rna_tf32(v);
   return v;
 }
 
-__device__ __forceinline__ void tc_epilogue(const TcParams& p, uint32_t tmem_base, int tile0, int nt_here, int nb0, int warp,
-                                            int lane, long long out_base, uint32_t stg) {
-  const int quarter = warp & 3;
-  const int m = quarter * 32 + lane;
-  const int wi = m % p.bw;
-  const int hi = (m / p.bw) % p.bh;
-  const int ni = m / (p.bw * p.bh);
-  const int sub = lane >> 3, c4 = (lane & 7) * 4;       // transposed role: row (i*4 + sub) of the chunk, columns c4..c4+3
-  for (int tl = 0; tl < nt_here; ++tl) {
-    int ow0, oh0, n0;
-    tc_tile_origin(p, tile0 + tl, ow0, oh0, n0);
-    // rows beyond the box (stale smem) and pixels outside the grid are computed but never stored
-    const bool row_ok = m < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.img_h && ow0 + wi < p.img_w;
-    // element offset of this row's first column in `out` (residual / mask share the output's geometry)
+// Epilogue of one pixel tile from the accumulator fragment of this thread: rows m and m + 8 of the tile, columns
+// 8j + 2 (lane % 4) + {0, 1}.  A quad of lanes writes 32 contiguous bytes of one output row.  Rows beyond the box (stale
+// smem) and pixels outside the grid are computed but never stored.
+template <int BN>
+__device__ __forceinline__ void tc_epilogue(const TcParams& p, const float* acc, int tile, int nb0, int wg, int warp, int lane,
+                                            long long out_base) {
+  int ow0, oh0, n0;
+  tc_tile_origin(p, tile, ow0, oh0, n0);
+  const int c2 = (lane & 3) * 2;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
+    const int wi = m % p.bw;
+    const int hi = (m / p.bw) % p.bh;
+    const int ni = m / (p.bw * p.bh);
+    if (!(m < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.img_h && ow0 + wi < p.img_w)) continue;
     const long long roff = out_base + (long long)(n0 + ni) * p.s_n + (long long)(oh0 + hi) * p.s_h +
                            (long long)(ow0 + wi) * p.s_w + nb0;
-    const uint32_t okmask = __ballot_sync(0xffffffffu, row_ok);
-    long long roffs[8];
-    if (stg) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) roffs[i] = __shfl_sync(0xffffffffu, roff, i * 4 + sub);
-    }
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(tl * p.bn);
-    // two warps share a lane quarter: the first takes the lower half of the 32-column chunks, the second the rest
-    const int nchunks = p.bn / 32, csplit = (nchunks + 1) / 2;
-    const int cbeg = (warp - 2) < 4 ? 0 : csplit * 32, cend = (warp - 2) < 4 ? csplit * 32 : p.bn;
-    for (int c0 = cbeg; c0 < cend; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(taddr + (uint32_t)c0, r);
-      const bool whole = nb0 + c0 + 32 <= p.cout && (p.cout & 3) == 0;      // warp-uniform
-      if (whole && stg) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          sts128(stg + lane * TC_EPI_ROW_BYTES + j * 16,
-                 make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                             __uint_as_float(r[4 * j + 3])));
-        __syncwarp();
-        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias) bv = *reinterpret_cast<const float4*>(p.bias + nb0 + c0 + c4);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 v = lds128(stg + (i * 4 + sub) * TC_EPI_ROW_BYTES + c4 * 4);
-          if ((okmask >> (i * 4 + sub)) & 1u) {
-            const long long off = roffs[i] + c0 + c4;
-            *reinterpret_cast<float4*>(p.out + off) = tc_epilogue_math(p, v, bv, off);
-          }
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = j * 8 + c2;
+      if (nb0 + c >= p.cout) continue;
+      float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      const long long off = roff + c;
+      if (p.vec2) {
+        if (p.bias) { const float2 b = *reinterpret_cast<const float2*>(p.bias + nb0 + c); v.x += b.x; v.y += b.y; }
+        if (p.residual) { const float2 r = *reinterpret_cast<const float2*>(p.residual + off); v.x += r.x; v.y += r.y; }
+        if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+        if (p.mask) {
+          const float2 mv = *reinterpret_cast<const float2*>(p.mask + off);
+          v.x = mv.x > 0.f ? v.x : p.mask_leak * v.x; v.y = mv.y > 0.f ? v.y : p.mask_leak * v.y;
         }
-        __syncwarp();
-      } else if (whole) {
-        if (row_ok) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                         __uint_as_float(r[j + 3]));
-            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias) bv = *reinterpret_cast<const float4*>(p.bias + nb0 + c0 + j);
-            *reinterpret_cast<float4*>(p.out + roff + c0 + j) = tc_epilogue_math(p, v, bv, roff + c0 + j);
-          }
-        }
-      } else if (row_ok) {      // thin / padded tile (e.g. the 256->3 image conv): only the first `cout` columns exist
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (nb0 + c0 + j < p.cout) {
-            float v = __uint_as_float(r[j]);
-            if (p.bias) v += p.bias[nb0 + c0 + j];
-            if (p.residual) v += p.residual[roff + c0 + j];
-            if (p.relu) v = fmaxf(v, 0.f);
-            if (p.mask) v = p.mask[roff + c0 + j] > 0.f ? v : p.mask_leak * v;
-            if (p.round_out) v = rna_tf32(v);
-            p.out[roff + c0 + j] = v;
-          }
-        }
+        if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
+        *reinterpret_cast<float2*>(p.out + off) = v;
+      } else {        // odd column count or odd row offsets (e.g. the 256->3 image conv): element by element
+        p.out[off] = tc_epilogue_one(p, v.x, nb0 + c, off);
+        if (nb0 + c + 1 < p.cout) p.out[off + 1] = tc_epilogue_one(p, v.y, nb0 + c + 1, off + 1);
       }
     }
   }
 }
 
-__global__ void __launch_bounds__(TC_THREADS, 2)
+// round this warpgroup's `bytes` of a tile (float4 per thread and sweep) to nearest TF32 in place
+__device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, int nthreads) {
+#pragma unroll 4
+  for (int i = q * 16; i < bytes; i += nthreads * 16) {
+    float4 v = lds128(base + i);
+    v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w);
+    sts128(base + i, v);
+  }
+}
+
+// CL = 2: the CTA runs in a cluster of two neighbouring pixel-tile groups that share the weight tile: each CTA loads half
+// of its rows and multicasts them to both, so a k-block costs each SM MT*16 KB + BN*64 B of L2 -> SM traffic instead of
+// MT*16 KB + BN*128 B (the kernel is bound by that feed at BN = 256).  A stage is refilled only when the consumers of BOTH
+// CTAs have released it (empty barrier count 2 x 2); the CTAs meet at cluster barriers after initialising the barriers and
+// before exiting, so no multicast or remote arrive ever targets a CTA that is not running.
+template <int BN, int MT, int CL>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][mt x A 16KB][B bn*128B] | barriers | tmem ptr
+  // carve: [stages][MT x A 16KB][B BN*128B] | barriers
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_bytes = p.bn * TC_BK * 4;
-  const int a_bytes = p.mt * TC_A_BYTES;
-  const int stage_bytes = a_bytes + b_bytes;
+  constexpr int b_bytes = BN * TC_BK * 4;
+  constexpr int a_bytes = MT * TC_A_BYTES;
+  constexpr int stage_bytes = a_bytes + b_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
-  uint64_t* ready_bar = full_bar + p.stages;
-  uint64_t* empty_bar = ready_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  uint64_t* empty_bar = full_bar + p.stages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tap0 = p.ph_tap0[blockIdx.z];
   const int num_kb = (p.ph_tap0[blockIdx.z + 1] - tap0) * p.kchunks;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
 
   // this CTA's pixel tiles: [tile0, tile0 + nt_here).  They all multiply the same weight tile, which is therefore
-  // fetched from L2 once per k-block for mt*128 pixels: the kernel is bound by L2->SM bytes per MMA, not by HBM.
-  const int tile0 = blockIdx.x * p.mt;
-  const int nt_here = min(p.mt, p.tiles_total - tile0);
-  auto tile_origin = [&](int i, int& ow0, int& oh0, int& n0) { tc_tile_origin(p, tile0 + i, ow0, oh0, n0); };
-  const int nb0 = blockIdx.y * p.bn;          // first output channel of this CTA
+  // fetched from L2 once per k-block for MT*128 pixels.  (A cluster's second CTA may lie past the last tile: nt_here = 0.)
+  const int tile0 = blockIdx.x * MT;
+  const int nt_here = max(0, min(MT, p.tiles_total - tile0));
+  const int nb0 = blockIdx.y * BN;          // first output channel of this CTA
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_as.m[0]) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < p.stages; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&ready_bar[s], TC_RWARPS);      // one arrive per rounding warp
-        mbar_init(&empty_bar[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2 * CL);            // one arrive per consumer warpgroup of every CTA that fills the stage
     }
-    __syncwarp();
-    // TMEM: 256 fp32 columns x 128 lanes for the accumulator
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
+  if (CL == 2) cluster_sync_all(); else __syncthreads();
 
-  if (warp == 0) {
+  if (warp == TC_CWARPS) {
     // ===== TMA producer =====
     if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_as.m[0]) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -263,292 +197,120 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
         mbar_expect_tx(&full_bar[stage], (uint32_t)(nt_here * p.rows_used * TC_BK * 4 + b_bytes));
         int ow0, oh0, n0;
         for (int i = 0; i < nt_here; ++i) {
-          tile_origin(i, ow0, oh0, n0);
+          tc_tile_origin(p, tile0 + i, ow0, oh0, n0);
           tma_load_4d(sa + i * TC_A_BYTES, &tm_as.m[p.amap[tap]], &full_bar[stage], kc * TC_BK, ow0 + p.off_w[tap],
                       oh0 + p.off_h[tap], n0);
         }
-        tile_origin(0, ow0, oh0, n0);           // batched GEMM: all tiles of a CTA lie in one image (host guarantees)
-        tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
+        if (CL == 2) {          // this CTA's half of the weight rows, into both CTAs (no batched GEMM here)
+          tma_load_3d_multicast(sb + rank * (BN / 2) * 128, &tm_b, &full_bar[stage], kc * TC_BK, nb0 + (int)rank * (BN / 2),
+                                p.wtap[tap], (uint16_t)3);
+        } else {
+          tc_tile_origin(p, tile0, ow0, oh0, n0);   // batched GEMM: all tiles of a CTA lie in one image (host guarantees)
+          tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
+        }
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 (1<<4), A=TF32 (2<<7), B=TF32 (2<<10), K-major A/B,
-    // N>>3 at [17,23), M>>4 at [24,29)
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-    int stage = 0;
+  } else {
+    // ===== consumer warpgroups =====
+    const int wg = warp >> 2;
+    const int q = threadIdx.x & 127;
+    float acc[MT][BN / 2];
+#pragma unroll
+    for (int t = 0; t < MT; ++t)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[t][i] = 0.f;
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(p.round_a ? &ready_bar[stage] : &full_bar[stage], phase);   // pre-rounded operands: straight from TMA
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-        const uint32_t b_addr = a_addr + a_bytes;
-        for (int i = 0; i < nt_here; ++i) {
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {     // UMMA_K = 8 for tf32: 32 B per step inside the 128 B swizzle row
-            umma_tf32(tmem_base + (uint32_t)(i * p.bn), make_desc(a_addr + i * TC_A_BYTES + k * 32), make_desc(b_addr + k * 32),
-                      idesc, (kb | k) ? 1u : 0u);
-          }
-        }
-        umma_commit(&empty_bar[stage]);              // frees the smem slot when these MMAs retire
-        if (kb == num_kb - 1) umma_commit(tmem_full_bar);
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + wg * TC_WG_A_BYTES;
+      const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + a_bytes;
+      if (p.round_a) {
+        for (int tl = 0; tl < nt_here; ++tl) tc_round_smem(a_addr + tl * TC_A_BYTES, TC_WG_A_BYTES, q, 128);
+        fence_proxy_async();
+        named_bar(1 + wg, 128);
       }
-      __syncwarp();
+#pragma unroll
+      for (int t = 0; t < MT; ++t)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+      wgmma_fence();
+      // every one of the MT tiles is multiplied (a tile past the grid's end holds stale rows that are never stored): one
+      // unconditional chain of MMAs
+#pragma unroll
+      for (int t = 0; t < MT; ++t) {
+#pragma unroll
+        for (int k = 0; k < TC_BK / 8; ++k)     // K = 8 for tf32: 32 B per step inside the 128 B swizzle row
+          wgmma_tf32<BN>(acc[t], make_desc(a_addr + t * TC_A_BYTES + k * 32), make_desc(b_addr + k * 32));
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                               // the previous k-block's MMAs have retired: free its stage
+#pragma unroll
+      for (int t = 0; t < MT; ++t)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+      if (prev >= 0 && q == 0) {
+        mbar_arrive(&empty_bar[prev]);
+        if (CL == 2) mbar_arrive_cluster(&empty_bar[prev], rank ^ 1);
+      }
+      prev = stage;
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // ===== warps 2..9: round A to nearest TF32 in smem, then epilogue =====
-    const int q = threadIdx.x - 64;                  // 0..255
-    if (p.round_a) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        uint32_t a4 = smem_u32(smem + stage * stage_bytes) + q * 16;
-        for (int tl = 0; tl < nt_here; ++tl, a4 += TC_A_BYTES) {
-          float4 v[TC_A_BYTES / 16 / (32 * TC_RWARPS)];       // 1024 float4 / 256 threads = 4 each, loads first
+    wgmma_wait<0>();
 #pragma unroll
-          for (int i = 0; i < TC_A_BYTES / 16 / (32 * TC_RWARPS); ++i) v[i] = lds128(a4 + i * (512 * TC_RWARPS));
+    for (int t = 0; t < MT; ++t) {
 #pragma unroll
-          for (int i = 0; i < TC_A_BYTES / 16 / (32 * TC_RWARPS); ++i) {
-            v[i].x = rna_tf32(v[i].x); v[i].y = rna_tf32(v[i].y); v[i].z = rna_tf32(v[i].z); v[i].w = rna_tf32(v[i].w);
-            sts128(a4 + i * (512 * TC_RWARPS), v[i]);
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (UMMA) reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&ready_bar[stage]);
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
+      for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+      if (t < nt_here) tc_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z]);
     }
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    tc_epilogue(p, tmem_base, tile0, nt_here, nb0, warp, lane, p.ph_base[blockIdx.z],
-                p.epi_stage ? smem_u32(smem) + (warp - 2) * TC_EPI_WARP_BYTES : 0u);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
-  }
-}
-
-// ---- CTA-pair variant (cta_group::2) ------------------------------------------------------------------------------------
-// The per-tap kernel above is bound by the shared-memory pipe of the SM: per k-block and CTA the TMA engine writes
-// mt*16 KB + bn*128 B while the tensor core reads every operand byte again (the weight tile once per pixel tile) —
-// ~160 B/clk against 128 B/clk at bn = 256, ~220 B/clk at bn = 128.  Here two CTAs of a cluster (the two SMs of a TPC)
-// share every weight tile: each CTA loads and holds HALF of its rows, one tcgen05.mma.cta_group::2 of M = 256 multiplies
-// the pixel tiles of both CTAs with the whole tile, so both the TMA fill and the UMMA reads of the weight operand halve
-// per SM.  Protocol (see tc_common.cuh): both CTAs run a TMA producer whose loads complete on the LEADER's `full`
-// barrier (count 2: the leader's expect_tx arrive for the bytes of both CTAs + the peer's remote arrive), the leader's
-// MMA warp issues for both and commits `empty` / `tmem_full` with a multicast arrive to both CTAs, each CTA's epilogue
-// warps drain their own TMEM half.  Operands that still need rounding are rounded by each CTA's warps 2..9 in its own
-// shared memory; they arrive on the leader's `ready` barrier (count 2 x 8 warps).
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 2)
-conv_tc_pair_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_half_bytes = (p.bn / 2) * TC_BK * 4;
-  const int a_bytes = p.mt * TC_A_BYTES;
-  const int stage_bytes = a_bytes + b_half_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
-  uint64_t* ready_bar = full_bar + p.stages;
-  uint64_t* empty_bar = ready_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int tap0 = p.ph_tap0[blockIdx.z];
-  const int num_kb = (p.ph_tap0[blockIdx.z + 1] - tap0) * p.kchunks;
-  const int tile0 = blockIdx.x * p.mt;          // tiles beyond tiles_total are all-zero boxes whose rows are never stored
-  const int nb0 = blockIdx.y * p.bn;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_as.m[0]) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < p.stages; ++s) {
-        mbar_init(&full_bar[s], p.round_a ? 1 : 2);      // pair mode: leader's expect_tx arrive + the peer's arrive
-        mbar_init(&ready_bar[s], 2 * TC_RWARPS);         // the rounding warps of both CTAs
-        mbar_init(&empty_bar[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  cluster_sync_all();                                    // barriers of both CTAs initialised before any remote arrive / TMA
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===== TMA producer (both CTAs): own pixel tiles + own half of the weight tile, completing on the leader's barrier =====
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int tl = kb / p.kchunks, kc = kb - tl * p.kchunks, tap = tap0 + tl;
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * stage_bytes;
-        uint8_t* sb = sa + a_bytes;
-        const uint32_t own_bytes = (uint32_t)(p.mt * p.rows_used * TC_BK * 4 + b_half_bytes);
-        int ow0, oh0, n0;
-        if (p.round_a) {
-          // the operand is rounded in shared memory first: every CTA completes its loads on its OWN barrier, its rounding
-          // warps wait there and then arrive on the leader's `ready` barrier, which is what the MMA warp waits for
-          mbar_expect_tx(&full_bar[stage], own_bytes);
-          for (int i = 0; i < p.mt; ++i) {
-            tc_tile_origin(p, tile0 + i, ow0, oh0, n0);
-            tma_load_4d(sa + i * TC_A_BYTES, &tm_as.m[p.amap[tap]], &full_bar[stage], kc * TC_BK, ow0 + p.off_w[tap],
-                        oh0 + p.off_h[tap], n0);
-          }
-          tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0 + (int)rank * (p.bn / 2), p.wtap[tap]);
-        } else {
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * own_bytes);
-          else mbar_arrive_cluster(&full_bar[stage], 0);
-          for (int i = 0; i < p.mt; ++i) {
-            tc_tile_origin(p, tile0 + i, ow0, oh0, n0);
-            tma_load_4d_pair(sa + i * TC_A_BYTES, &tm_as.m[p.amap[tap]], &full_bar[stage], kc * TC_BK, ow0 + p.off_w[tap],
-                             oh0 + p.off_h[tap], n0);
-          }
-          tma_load_3d_pair(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0 + (int)rank * (p.bn / 2), p.wtap[tap]);
-        }
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer: the leader only, for both CTAs =====
-    if (leader) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(p.round_a ? &ready_bar[stage] : &full_bar[stage], phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) {
-          const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-          const uint32_t b_addr = a_addr + a_bytes;
-          for (int i = 0; i < p.mt; ++i) {
-#pragma unroll
-            for (int k = 0; k < TC_BK / 8; ++k)
-              umma_tf32_pair(tmem_base + (uint32_t)(i * p.bn), make_desc(a_addr + i * TC_A_BYTES + k * 32), make_desc(b_addr + k * 32),
-                             idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit_pair(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit_pair(tmem_full_bar);
-        }
-        __syncwarp();
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // ===== warps 2..9: round the own A tiles (operand not pre-rounded), then the epilogue of the own tiles =====
-    const int q = threadIdx.x - 64;
-    if (p.round_a) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);              // this CTA's own loads (local completion in rounding mode)
-        uint32_t a4 = smem_u32(smem + stage * stage_bytes) + q * 16;
-        for (int tl = 0; tl < p.mt; ++tl, a4 += TC_A_BYTES) {
-          float4 v[TC_A_BYTES / 16 / (32 * TC_RWARPS)];
-#pragma unroll
-          for (int i = 0; i < TC_A_BYTES / 16 / (32 * TC_RWARPS); ++i) v[i] = lds128(a4 + i * (512 * TC_RWARPS));
-#pragma unroll
-          for (int i = 0; i < TC_A_BYTES / 16 / (32 * TC_RWARPS); ++i) {
-            v[i].x = rna_tf32(v[i].x); v[i].y = rna_tf32(v[i].y); v[i].z = rna_tf32(v[i].z); v[i].w = rna_tf32(v[i].w);
-            sts128(a4 + i * (512 * TC_RWARPS), v[i]);
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(&ready_bar[stage], 0);
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    tc_epilogue(p, tmem_base, tile0, p.mt, nb0, warp, lane, p.ph_base[blockIdx.z],
-                p.epi_stage ? smem_u32(smem) + (warp - 2) * TC_EPI_WARP_BYTES : 0u);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  cluster_sync_all();                                    // the peer's TMEM / barriers stay alive until both CTAs are done
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
-  }
+  if (CL == 2) cluster_sync_all();
 }
 
 // ---- halo variant ------------------------------------------------------------------------------------------------
-// 3x3 stride-1 convolutions (forward and input gradient) are bound by the L2 -> shared-memory operand feed, not by the
-// tensor pipe (DESIGN.md section 3): per 32-channel k-block a CTA pulls 16 KB of activations per pixel tile for every one
-// of the nine taps although the nine boxes overlap almost completely.  Here the three taps of one kernel COLUMN share a
-// single TMA box of bh + 2 image rows; the vertical shift of a tap is a descriptor start-address offset of bw pixel rows
-// (a multiple of 1024 B, so the 128B-swizzle phase is unchanged).  The activation operand is fetched 3 x (bh+2)/bh times
-// per chunk instead of 9 x (x1.5 instead of x9 at 4-row tiles), which also halves the in-smem rounding work of operands
-// that are not pre-rounded.  Activations and weights run in two rings of their own (a halo box lives for three k-blocks).
-// Up to four pixel tiles per CTA share each weight tile (mt x bn <= 512 TMEM columns), one CTA per SM.
+// 3x3 stride-1 convolutions whose activation operand still has to be rounded: per 32-channel k-block a CTA would pull
+// 16 KB of activations per pixel tile for every one of the nine taps although the nine boxes overlap almost completely.
+// Here the three taps of one kernel COLUMN share a single TMA box of bh + 2 image rows; the vertical shift of a tap is a
+// descriptor start-address offset of bw pixel rows (a multiple of 1024 B, so the 128B-swizzle phase is unchanged).  The
+// activation operand is fetched 3 x (bh+2)/bh times per chunk instead of 9 x, which also cuts the in-smem rounding work
+// by the same factor.  Activations and weights run in two rings of their own (a halo box lives for three k-blocks).
+template <int BN, int MT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_bytes = p.bn * TC_BK * 4;
-  const int a_stage = p.mt * p.a_halo_bytes;
+  constexpr int b_bytes = BN * TC_BK * 4;
+  const int a_stage = MT * p.a_halo_bytes;
   uint8_t* smem_b = smem + p.sa_stages * a_stage;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem_b + p.sb_stages * b_bytes);
-  uint64_t* a_ready = a_full + p.sa_stages;
-  uint64_t* a_empty = a_ready + p.sa_stages;
+  uint64_t* a_empty = a_full + p.sa_stages;
   uint64_t* b_full = a_empty + p.sa_stages;
   uint64_t* b_empty = b_full + p.sb_stages;
-  uint64_t* tmem_full_bar = b_empty + p.sb_stages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tile0 = blockIdx.x * p.mt;
-  const int nt_here = min(p.mt, p.tiles_total - tile0);
-  const int nb0 = blockIdx.y * p.bn;
+  const int tile0 = blockIdx.x * MT;
+  const int nt_here = min(MT, p.tiles_total - tile0);
+  const int nb0 = blockIdx.y * BN;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < p.sa_stages; ++s) {
-        mbar_init(&a_full[s], 1);
-        mbar_init(&a_ready[s], TC_RWARPS);
-        mbar_init(&a_empty[s], 1);
-      }
-      for (int s = 0; s < p.sb_stages; ++s) {
-        mbar_init(&b_full[s], 1);
-        mbar_init(&b_empty[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.sa_stages; ++s) {
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], 2);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    for (int s = 0; s < p.sb_stages; ++s) {
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], 2);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == TC_CWARPS) {
     // ===== TMA producer: per (channel chunk, tap column) one halo box per tile, then the hnv weight tiles =====
     if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;
       for (int kc = 0; kc < p.kchunks; ++kc) {
@@ -571,72 +333,67 @@ conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-    int sa = 0, sb = 0;
-    uint32_t pa = 0, pb = 0;
-    const uint32_t tap_shift = (uint32_t)(p.bw * 128);          // one image row of the box = bw pixel rows of 128 B
-    for (int kc = 0; kc < p.kchunks; ++kc) {
-      for (int g = 0; g < p.hg; ++g) {
-        mbar_wait(p.round_a ? &a_ready[sa] : &a_full[sa], pa);
-        const uint32_t a_addr = smem_u32(smem + sa * a_stage);
-        for (int t = 0; t < p.hnv; ++t) {
-          mbar_wait(&b_full[sb], pb);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          if (lane == 0) {
-            const uint32_t b_addr = smem_u32(smem_b + sb * b_bytes);
-            const uint32_t first = (kc | g | t) ? 1u : 0u;
-            for (int i = 0; i < nt_here; ++i) {
-#pragma unroll
-              for (int k = 0; k < TC_BK / 8; ++k)
-                umma_tf32(tmem_base + (uint32_t)(i * p.bn), make_desc(a_addr + i * p.a_halo_bytes + t * tap_shift + k * 32),
-                          make_desc(b_addr + k * 32), idesc, (first | (uint32_t)k) ? 1u : 0u);
-            }
-            umma_commit(&b_empty[sb]);
-            if (t == p.hnv - 1) umma_commit(&a_empty[sa]);
-            if (kc == p.kchunks - 1 && g == p.hg - 1 && t == p.hnv - 1) umma_commit(tmem_full_bar);
-          }
-          __syncwarp();
-          if (++sb == p.sb_stages) { sb = 0; pb ^= 1; }
-        }
-        if (++sa == p.sa_stages) { sa = 0; pa ^= 1; }
-      }
-    }
-  } else {
-    // ===== warps 2..9: round the halo boxes to nearest TF32 in smem (operand not pre-rounded), then the epilogue =====
-    if (p.round_a) {
-      const int q = threadIdx.x - 64;
-      const int n16 = p.a_box_bytes / 16;            // float4s per box (a multiple of 32 * TC_RWARPS, host-checked)
-      int sa = 0;
-      uint32_t pa = 0;
-      for (int it = 0; it < p.kchunks * p.hg; ++it) {
-        mbar_wait(&a_full[sa], pa);
-        for (int tl = 0; tl < nt_here; ++tl) {
-          const uint32_t a4 = smem_u32(smem + sa * a_stage + tl * p.a_halo_bytes);
-#pragma unroll 2
-          for (int i = q; i < n16; i += 32 * TC_RWARPS) {
-            float4 v = lds128(a4 + i * 16);
-            v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w);
-            sts128(a4 + i * 16, v);
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[sa]);
-        if (++sa == p.sa_stages) { sa = 0; pa ^= 1; }
-      }
-    }
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    tc_epilogue(p, tmem_base, tile0, nt_here, nb0, warp, lane, p.base,
-                p.epi_stage ? smem_u32(smem) + (warp - 2) * TC_EPI_WARP_BYTES : 0u);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
+
+  // ===== consumer warpgroups =====
+  const int wg = warp >> 2;
+  float acc[MT][BN / 2];
+#pragma unroll
+  for (int t = 0; t < MT; ++t)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[t][i] = 0.f;
+  const uint32_t tap_shift = (uint32_t)(p.bw * 128);          // one image row of the box = bw pixel rows of 128 B
+  int sa = 0, sb = 0, prev_a = -1, prev_b = -1;
+  uint32_t pa = 0, pb = 0;
+  for (int kc = 0; kc < p.kchunks; ++kc) {
+    for (int g = 0; g < p.hg; ++g) {
+      mbar_wait(&a_full[sa], pa);
+      const uint32_t a_addr = smem_u32(smem + sa * a_stage);
+      if (p.round_a) {          // the box rows are shared by both warpgroups: round it together, then sync the two
+        for (int tl = 0; tl < nt_here; ++tl) tc_round_smem(a_addr + tl * p.a_halo_bytes, p.a_box_bytes, threadIdx.x, 256);
+        fence_proxy_async();
+        named_bar(1, 256);
+      }
+      for (int t = 0; t < p.hnv; ++t) {
+        mbar_wait(&b_full[sb], pb);
+        const uint32_t b_addr = smem_u32(smem_b + sb * b_bytes);
+#pragma unroll
+        for (int u = 0; u < MT; ++u)
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
+        wgmma_fence();
+#pragma unroll
+        for (int u = 0; u < MT; ++u) {
+#pragma unroll
+          for (int k = 0; k < TC_BK / 8; ++k)
+            wgmma_tf32<BN>(acc[u], make_desc(a_addr + u * p.a_halo_bytes + t * tap_shift + wg * TC_WG_A_BYTES + k * 32),
+                           make_desc(b_addr + k * 32));
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+#pragma unroll
+        for (int u = 0; u < MT; ++u)
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
+        // the previous group of MMAs has retired: release its weight tile (and its halo box after a column's last tap)
+        if ((threadIdx.x & 127) == 0) {
+          if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
+          if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+        }
+        prev_b = sb;
+        prev_a = (t == p.hnv - 1) ? sa : -1;
+        if (++sb == p.sb_stages) { sb = 0; pb ^= 1; }
+      }
+      if (++sa == p.sa_stages) { sa = 0; pa ^= 1; }
+    }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int t = 0; t < MT; ++t) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+    if (t < nt_here) tc_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.base);
   }
 }
 
@@ -670,7 +427,7 @@ inline void tc_geometry(int n, int h, int w, int* bw, int* bh, int* bni, int* tw
   *tn = (n + *bni - 1) / *bni;
 }
 
-inline int tc_pick_bn(int ncols_pad) {     // largest UMMA N <= 256 (multiple of 32) that divides the padded column count
+inline int tc_pick_bn(int ncols_pad) {     // largest wgmma N <= 256 (multiple of 32) that divides the padded column count
   if (ncols_pad <= 256) return ncols_pad;
   for (int b = 256; b >= 32; b -= 32)
     if (ncols_pad % b == 0) return b;
@@ -690,6 +447,66 @@ inline int tc_pick_bn_occupancy(int ncols_pad, long long tiles_m, int sms) {
     if (tiles_m * (ncols_pad / b) >= sms) break;
   }
   return pick;
+}
+
+
+// every output row of the launch starts at an even element offset and the column count is even: float2 epilogue
+inline int tc_vec2(const TcParams& p) {
+  long long odd = p.cout | p.s_n | p.s_h | p.s_w | p.base;
+  for (int i = 0; i < p.nphases; ++i) odd |= p.ph_base[i];
+  return (odd & 1) ? 0 : 1;
+}
+
+// kind: 0 plain kernel, 1 plain kernel in two-CTA clusters (grid.x even; `b` maps half of the weight tile), 2 halo kernel
+template <int BN, int MT>
+int tc_launch_t(cgan_ctx* ctx, int kind, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& a1,
+                const CUtensorMap& b, const TcParams& p) {
+  static bool attr_set[3] = {false, false, false};
+  if (kind == 2) {
+    if (!attr_set[2]) {
+      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_halo_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set[2] = true;
+    }
+    conv_tc_halo_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(a1, b, p);
+  } else if (kind == 1) {
+    if (!attr_set[1]) {
+      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set[1] = true;
+    }
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = grid;
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = ctx->stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    CGAN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MT, 2>, as, b, p));
+  } else {
+    if (!attr_set[0]) {
+      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set[0] = true;
+    }
+    conv_tc_kernel<BN, MT, 1><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p);
+  }
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+// the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS
+int tc_launch(cgan_ctx* ctx, int kind, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& a1, const CUtensorMap& b,
+              const TcParams& p) {
+#define TC_CASE(BN, MT) \
+  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, kind, grid, smem, as, a1, b, p);
+  TC_CASE(32, 1) TC_CASE(64, 1) TC_CASE(96, 1) TC_CASE(128, 1) TC_CASE(160, 1) TC_CASE(192, 1) TC_CASE(224, 1)
+  TC_CASE(256, 1) TC_CASE(32, 2) TC_CASE(64, 2) TC_CASE(96, 2) TC_CASE(128, 2)
+#undef TC_CASE
+  return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: no kernel for this column tile / pixel-tile count%s", "cgan_conv_tc");
 }
 
 }  // namespace
@@ -757,7 +574,6 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   p.rows_used = p.bw * p.bh * p.bni;
   p.img_n = n; p.img_h = gh; p.img_w = gw;
   p.relu = relu;
-  p.epi_stage = ctx->tc_epi;          // every ring below holds >= 40 KB >= 8 warps x TC_EPI_WARP_BYTES
   p.round_a = (ex && ex->a_prerounded) ? 0 : 1;
   if (ex) {
     p.round_out = ex->round_out; p.residual = ex->residual; p.mask = ex->mask; p.mask_leak = ex->mask_leak;
@@ -788,10 +604,9 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   }
 
   // ---- halo variant: three taps of a kernel column share one (bh+2)-row activation box --------------------------------
-  // Measured (round 2, profiles/r2_microbench.txt): with a pre-rounded operand the per-tap kernel is bound by the
-  // shared-memory pipe (TMA fills + UMMA operand reads), not by the L2 feed, and the halo variant (one CTA per SM) is no
-  // faster (256 -> 256) or slower (128 -> 128, which runs two per-tap CTAs per SM); it wins 8 % when the operand still
-  // has to be rounded in shared memory (half the rounding work).  CGAN_OPT_TC_HALO = 2 forces it everywhere (tests).
+  // Used where the activation operand still has to be rounded in shared memory (the halo box cuts that work 9 -> 3 x
+  // (bh+2)/bh per chunk); a pre-rounded operand streams through the per-tap kernel.  CGAN_OPT_TC_HALO = 2 forces it
+  // everywhere (tests).
   const bool halo_wanted = ctx->tc_halo == 2 || (ctx->tc_halo == 1 && p.round_a && ncols_pad >= 256);
   if (halo_wanted && p.nphases == 1 && nviews == 1 && wimg_stride == 0 && ntaps == 9 && gh == h && gw == w && !view_phase_of) {
     int hbw = 0, hbh = 0;
@@ -834,26 +649,24 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
       p.a_box_bytes = (hbh + 2) * hbw * 128;
       p.a_halo_bytes = (p.a_box_bytes + 1023) / 1024 * 1024;
       const int b_bytes = p.bn * TC_BK * 4;
-      // pixel tiles per CTA (they share every weight tile): as many as the 512 TMEM columns hold, while two waves of CTAs
-      // remain and the weight ring keeps >= 4 stages (a k-block of mt tiles is ~mt*bn/2 clocks of MMA; the ring has to
-      // cover the L2 latency of ~2-4 k-blocks).  The activation ring has two stages, each good for three k-blocks.
+      // pixel tiles per CTA (they share every weight tile): as many as the accumulator registers hold (mt x bn <= 256),
+      // while two waves of CTAs remain and the weight ring keeps >= 4 stages.  The activation ring has two stages, each
+      // good for three k-blocks.
       const int budget = 227 * 1024 - 1024 - 512;
-      const int mt_cap = ctx->tc_mt_max >= 2 ? 4 : 1;
+      const int mt_cap = ctx->tc_mt_max >= 2 ? 2 : 1;
       p.sa_stages = 2;
       p.mt = 1;
       for (int m = mt_cap; m >= 2; --m) {
-        if (m * p.bn > 512 || tiles_total * ncol_tiles < 2ll * m * ctx->num_sms) continue;
+        if (m * p.bn > TC_ACC_COLS || tiles_total * ncol_tiles < 2ll * m * ctx->num_sms) continue;
         if ((budget - p.sa_stages * m * p.a_halo_bytes) / b_bytes < 4) continue;
         p.mt = m;
         break;
       }
       p.sb_stages = (budget - p.sa_stages * p.mt * p.a_halo_bytes) / b_bytes;
       if (p.sb_stages > 8) p.sb_stages = 8;
-      ok = p.sb_stages >= 2 && (p.a_box_bytes / 16) % (32 * TC_RWARPS) == 0;
+      ok = p.sb_stages >= 2;
       if (ok) {
         p.tiles_total = (int)tiles_total;
-        p.tmem_cols = 32;
-        while (p.tmem_cols < p.mt * p.bn) p.tmem_cols *= 2;
         CUtensorMap tm_a, tm_bh;
         if (!make_act_map(&tm_a, in + view_off[0], kdim, w, h, n, in_sw, in_sh, in_sn, hbw, hbh + 2, 1))
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A halo) failed%s", "cgan_conv_tc");
@@ -864,16 +677,12 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
         if (enc(&tm_bh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
+        p.vec2 = tc_vec2(p);
         size_t smem = (size_t)p.sa_stages * p.mt * p.a_halo_bytes + (size_t)p.sb_stages * b_bytes + 1024 + 512;
-        static bool halo_attr_set = false;
-        if (!halo_attr_set) {
-          CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-          halo_attr_set = true;
-        }
         dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles);
-        conv_tc_halo_kernel<<<grid, TC_THREADS, smem, ctx->stream>>>(tm_a, tm_bh, p);
-        CGAN_LAUNCHED(ctx);
-        return CGAN_OK;
+        AMaps unused;
+        memset(&unused, 0, sizeof(unused));
+        return tc_launch(ctx, 2, grid, smem, unused, tm_a, tm_bh, p);
       }
     }
     // not eligible after all: restore the standard geometry
@@ -904,88 +713,38 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
   }
-  // ---- CTA-pair variant: two SMs share every weight tile (cta_group::2) --------------------------------------------------
-  if (ctx->tc_pair && wimg_stride == 0 && ncols_pad % 64 == 0) {
-    const long long tiles_total = (long long)p.tiles_w * p.tiles_h * tiles_n;
-    TcParams q = p;
-    q.bn = tc_pick_bn(ncols_pad);                 // widest column tile: the pair is about weight-tile reuse
-    const int ncol_tiles = ncols_pad / q.bn;
-    q.mt = 1;
-    for (int m = 4; m >= 2; --m)
-      if (m * q.bn <= 512 && tiles_total * ncol_tiles * q.nphases >= 2ll * m * ctx->num_sms) { q.mt = m; break; }
-    if (ctx->tc_mt_max < 2) q.mt = 1;
-    if (ctx->tc_pair_mt > 0 && ctx->tc_pair_mt * q.bn <= 512) q.mt = ctx->tc_pair_mt;       // experiment knob (CGAN_TC_PAIR_MT)
-    const long long groups = (tiles_total + q.mt - 1) / q.mt;
-    if (q.bn % 32 == 0 && q.bn >= 64 && groups * ncol_tiles * q.nphases >= ctx->num_sms) {
-      const size_t stage_bytes = (size_t)q.mt * TC_A_BYTES + (size_t)(q.bn / 2) * TC_BK * 4;
-      // two CTA pairs per SM pair when the accumulators take at most half of the TMEM: one pair's epilogue then overlaps
-      // the other's main loop
-      const bool two_per_sm = q.mt * q.bn <= 256;
-      q.stages = (int)(((two_per_sm ? 113 : 227) * 1024 - 1024 - 512) / stage_bytes);
-      if (q.stages > 6) q.stages = 6;
-      if (q.stages >= 2) {
-        q.tiles_total = (int)tiles_total;
-        q.tmem_cols = 32;
-        while (q.tmem_cols < q.mt * q.bn) q.tmem_cols *= 2;
-        AMaps tma;
-        memset(&tma, 0, sizeof(tma));
-        for (int v = 0; v < 4; ++v) {
-          int vv = v < nviews ? v : 0;
-          int vh = h, vw = w;
-          if (nviews == 4 && view_phase_of) { vh = (view_phase_of[0] - (vv >> 1) + 1) / 2; vw = (view_phase_of[1] - (vv & 1) + 1) / 2; }
-          if (vh < 1 || vw < 1) { vh = h; vw = w; vv = 0; }
-          if (!make_act_map(&tma.m[v], in + view_off[vv], kdim, vw, vh, n, in_sw, in_sh, in_sn, q.bw, q.bh, q.bni))
-            return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A) failed%s", "cgan_conv_tc");
-        }
-        CUtensorMap tmb;
-        cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
-        cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
-        cuuint32_t box[3] = {TC_BK, (cuuint32_t)(q.bn / 2), 1};
-        cuuint32_t es[3] = {1, 1, 1};
-        if (enc(&tmb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-          return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B half) failed%s", "cgan_conv_tc");
-        size_t smem = (size_t)q.stages * stage_bytes + 1024 + 512;
-        static bool pair_attr_set = false;
-        if (!pair_attr_set) {
-          CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-          pair_attr_set = true;
-        }
-        dim3 grid((unsigned)((groups + 1) / 2 * 2), (unsigned)ncol_tiles, (unsigned)q.nphases);
-        conv_tc_pair_kernel<<<grid, TC_THREADS, smem, ctx->stream>>>(tma, tmb, q);
-        CGAN_LAUNCHED(ctx);
-        return CGAN_OK;
-      }
-    }
-  }
 
-  // Two CTAs per SM (each owns 256 of the 512 TMEM columns): one CTA's epilogue and prologue overlap the other's main
-  // loop, which matters for the short-K convolutions (3x3x128: 36 k-blocks).  ~110 KB of smem each.
-  // Pixel tiles per CTA: with mt = 2 the weight tile is fetched once for 256 pixels, which cuts the L2->SM bytes per MMA by
-  // a third (bn = 256: 96 -> 64 B/clk/SM against a ~43 B/clk/SM L2 budget).  bn = 256 then fills the TMEM (one CTA per SM),
-  // bn <= 128 keeps two CTAs per SM.  Only when enough CTAs remain to fill the machine.
+  // Pixel tiles per CTA: with mt = 2 the weight tile is fetched once for 256 pixels, which cuts the L2->SM bytes per MMA
+  // by a third; the accumulators (mt x bn columns) must fit the consumer registers, so only for bn <= 128, and only when
+  // enough CTAs remain to fill the machine.  Up to ~110 KB of smem per CTA when the tile is narrow, so that two CTAs
+  // share an SM and one's epilogue overlaps the other's main loop.
   const long long tiles_total = (long long)p.tiles_w * p.tiles_h * tiles_n;
   const int ncol_tiles = ncols_pad / p.bn;
   p.tiles_total = (int)tiles_total;
   p.mt = 1;
-  if (ctx->tc_mt_max >= 2 && tiles_total * ncol_tiles * p.nphases >= 4ll * ctx->num_sms &&
+  if (ctx->tc_mt_max >= 2 && 2 * p.bn <= TC_ACC_COLS && tiles_total * ncol_tiles * p.nphases >= 4ll * ctx->num_sms &&
       (wimg_stride == 0 || (p.tiles_w * p.tiles_h) % 2 == 0))
     p.mt = 2;
-  const bool two_ctas = p.mt * p.bn <= 256;
+  const bool two_ctas = p.mt * p.bn <= 128;
   const size_t stage_bytes = (size_t)p.mt * TC_A_BYTES + (size_t)p.bn * TC_BK * 4;
   p.stages = (int)(((two_ctas ? 110 : 220) * 1024) / stage_bytes);
   if (p.stages > TC_MAX_STAGES) p.stages = TC_MAX_STAGES;
   if (p.stages < 2) p.stages = 2;
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.mt * p.bn) p.tmem_cols *= 2;
+  p.vec2 = tc_vec2(p);
   size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles, (unsigned)p.nphases);
-  conv_tc_kernel<<<grid, TC_THREADS, smem, ctx->stream>>>(tm_as, tm_b, p);
-  CGAN_LAUNCHED(ctx);
-  return CGAN_OK;
+  // CGAN_OPT_TC_PAIR: neighbouring CTAs run as two-CTA clusters that share each weight tile through TMA multicast
+  if (ctx->tc_pair && wimg_stride == 0 && grid.x >= 2) {
+    CUtensorMap tm_bh;
+    cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
+    cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
+    cuuint32_t box[3] = {TC_BK, (cuuint32_t)(p.bn / 2), 1};
+    cuuint32_t es[3] = {1, 1, 1};
+    if (enc(&tm_bh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B half) failed%s", "cgan_conv_tc");
+    grid.x = (grid.x + 1) / 2 * 2;
+    return tc_launch(ctx, 1, grid, smem, tm_as, tm_bh, tm_bh, p);
+  }
+  return tc_launch(ctx, 0, grid, smem, tm_as, tm_b, tm_b, p);
 }

@@ -1,7 +1,7 @@
 // Exact-fp32 gather-GEMM family: conv2d fwd / dgrad / wgrad (implicit GEMM over NHWC + HWIO,
 // TF SAME padding, strides, fused zero-insertion upsampling) and plain/batched row-major GEMM.
 // This is math_mode 0: the bit-faithful fp32 contraction every shape can fall back to and the
-// on-device yard-stick for the tcgen05 path (conv_tc.cu).
+// on-device yard-stick for the tensor-core path (conv_tc.cu).
 //
 // Replaces: tf.nn.conv2d (arch_ops.py:568), its autodiff Conv2DBackpropInput/Filter,
 // tf.nn.conv2d_transpose (arch_ops.py:588-589), resnet_ops.unpool+conv (resnet_ops.py:122-130),
@@ -410,7 +410,7 @@ int cgan_conv2d_wgrad_simt(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   p.ldc = d->cout;
   p.vecA = (d->cin % 8 == 0) && al16(x);
   p.vecB = (d->cout % 8 == 0) && al16(dy);
-  // split-K so that the (tap,cin) x cout grid fills the 148 SMs about four times over
+  // split-K so that the (tap,cin) x cout grid fills the SMs about four times over
   long long tiles = (long long)cdiv(p.M, BM) * cdiv(p.N, p.N > 32 ? 128 : 32);
   int ktiles = cdiv(p.K, BK);
   int splits = (int)((4ll * ctx->num_sms + tiles - 1) / tiles);

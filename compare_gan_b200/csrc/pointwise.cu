@@ -28,7 +28,6 @@ int cgan_ctx_create(cgan_ctx** out, int device) {
   if (const char* e = getenv("CGAN_TC_MT")) c->tc_mt_max = atoi(e) >= 2 ? 2 : 1;
   c->tc_pair = 0;
   if (const char* e = getenv("CGAN_TC_PAIR")) c->tc_pair = atoi(e) ? 1 : 0;
-  if (const char* e = getenv("CGAN_TC_PAIR_MT")) c->tc_pair_mt = atoi(e);
   c->tc_epi = 1;
   if (const char* e = getenv("CGAN_TC_EPI")) c->tc_epi = atoi(e) ? 1 : 0;
   c->tc_halo = 1;
@@ -67,7 +66,7 @@ int cgan_ctx_reserve_workspace(cgan_ctx* ctx, size_t bytes) {
 
 int cgan_ctx_set_math_mode(cgan_ctx* ctx, int mode) {
   if (!ctx) return CGAN_ERR_ARG;
-  CGAN_REQUIRE(ctx, mode == 0 || mode == 1, "mode must be 0 (fp32 SIMT) or 1 (tcgen05 tf32)");
+  CGAN_REQUIRE(ctx, mode == 0 || mode == 1, "mode must be 0 (fp32 SIMT) or 1 (wgmma tf32)");
   ctx->math_mode = mode;
   return CGAN_OK;
 }

@@ -1,8 +1,9 @@
-// Shared PTX wrappers for the tcgen05 / TMA / mbarrier kernels (conv_tc.cu, wgrad_tc.cu).
+// Shared PTX wrappers for the wgmma / TMA / mbarrier kernels (conv_tc.cu, wgrad_tc.cu, attn_tc.cu).
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma_tf32.cuh"
 
 namespace tc {
 
@@ -41,30 +42,26 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
+// ---- warpgroup MMA (wgmma, sm_90a) -----------------------------------------------------------------------------------
+// K-major, 128B-swizzled shared-memory matrix descriptor (PTX ISA "Matrix Descriptor Format" for wgmma): start>>4 [0,14)
+// | LBO>>4 [16,30) (unused for swizzled K-major, 1) | SBO>>4 [32,46) = 1024 B between 8-row groups | layout SWIZZLE_128B = 1
+// [62,64).  The tile is what a TMA box of 32 fp32 channels with CU_TENSOR_MAP_SWIZZLE_128B writes: row r at r * 128 B,
+// its 16-byte chunks permuted by (r & 7).  K steps of 8 (32 B) advance the start address inside the swizzle row.
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) forms ------------------------------------------------------------------------------------
-// Two CTAs of one cluster (the two SMs of a TPC) execute ONE tcgen05.mma of M = 256: rows 0..127 come from the leader's
-// shared memory / accumulate in the leader's TMEM, rows 128..255 in the peer's; each CTA holds HALF of the B tile (N/2
-// rows).  Only the leader issues MMAs; TMA loads of both CTAs complete on the LEADER's mbarrier (its shared::cluster
-// address is the local one with the peer bit 24 cleared); tcgen05.commit multicasts its arrival to both CTAs.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
+// ---- two-CTA clusters sharing the weight tile (TMA multicast) ----------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
+// every thread of every CTA of the cluster
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -73,34 +70,35 @@ __device__ __forceinline__ void cluster_sync_all() {
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* map, uint64_t* leader_bar, int c0, int c1, int c2, int c3) {
+// the box lands at the same offset of every CTA in `mask`, completing bytes on each one's mbarrier at `bar`'s offset
+__device__ __forceinline__ void tma_load_3d_multicast(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
+                                                      uint16_t mask) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask) : "memory");
 }
-__device__ __forceinline__ void tma_load_3d_pair(void* dst, const CUtensorMap* map, uint64_t* leader_bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_pair(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrival on the barrier at this offset in BOTH CTAs of the pair once the MMAs issued so far have retired
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// barrier over `count` threads (named barrier `id`, 1..15)
+__device__ __forceinline__ void named_bar(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// generic-proxy writes to shared memory (operand rounding / transposition) become visible to the async proxy (wgmma)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// K-major 128B-swizzled tile (128-byte rows of 32 fp32): byte offset of element (row, k)
+__device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
+  return (uint32_t)(row * 128 + ((((k >> 2) ^ row) & 7) << 4) + (k & 3) * 4);
 }
 
 // explicit shared-space 128-bit accesses: a pointer carved out of the dynamic smem buffer compiles to GENERIC LD/ST
-// (ncu source page: LD.E.128 / ST.E.128 with long-scoreboard stalls); these are LDS.128 / STS.128
+// LD.E.128 / ST.E.128; these are LDS.128 / STS.128
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
@@ -116,20 +114,6 @@ __device__ __forceinline__ float rna_tf32(float x) {
   return __uint_as_float(u);
 }
 
-
-// tcgen05.ld 32 lanes x 32 columns (one fp32 accumulator row segment per thread)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,

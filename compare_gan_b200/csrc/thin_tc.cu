@@ -3,11 +3,11 @@
 // The first convolution of every discriminator (3 input channels), the last of every generator (3 output channels) and
 // Inception's stem are contractions over kh*kw*3 = 27 values per pixel: far too skinny for an implicit GEMM over
 // 32-channel k-blocks (the tap loop would move the 256-channel operand nine times for 3 output channels) and, as fp32
-// streaming kernels (thin.cu), bound by the FP32 pipe at 4-6x their HBM time (profiles/r2_launch_summary: 10 % of the
-// resnet_cifar10 cycle).  Here each becomes ONE dense 32-wide GEMM on the existing tcgen05 kernels plus a streaming pass:
+// streaming kernels (thin.cu), bound by the FP32 pipe at several times their HBM time.
+// Here each becomes ONE dense 32-wide GEMM on the existing wgmma kernels plus a streaming pass:
 //
-//   cin <= 4   forward   : P = patches(x) [pixels, 32]  ->  y  = P W            (1x1 tcgen05 conv, fused epilogue)
-//              filter    : dW = P^T dy                                            (tcgen05 filter-gradient kernel)
+//   cin <= 4   forward   : P = patches(x) [pixels, 32]  ->  y  = P W            (1x1 wgmma conv, fused epilogue)
+//              filter    : dW = P^T dy                                            (wgmma filter-gradient kernel)
 //              input grad: T = dy W^T [pixels, 32]      ->  dx = shift_add(T)
 //   cout <= 4  forward   : T = x W' [pixels, 32]        ->  y  = shift_add(T) + bias
 //              input grad: P = patches(dy)              ->  dx = P W'^T

@@ -1,4 +1,4 @@
-// tcgen05 filter-gradient kernel (math_mode 1):
+// Warpgroup-MMA (wgmma, sm_90a) filter-gradient kernel (math_mode 1):
 //
 //   dW[tap][ci][co] = sum_pixels  X[pixel + off(tap)][ci] * dY[pixel][co]
 //
@@ -6,11 +6,10 @@
 // channels contiguous): D[ci, co] += A[ci, pix] * B[pix, co].  Per k-block of 32 pixels, TMA brings
 //   * 4 boxes  [32 pixels x 32 ci]  of X  (shifted by the tap offset; SAME padding = TMA zero fill), and
 //   * N/32 boxes [32 pixels x 32 co] of dY
-// each box = 32 rows x 128 B.  For 32-bit MN-major operands the tensor core only accepts the SWIZZLE_128B_BASE32B
-// layout (cute Layout_MN_SW128_32B_Atom: Swizzle<2,5,2>, 128 B x 4-row atoms, 32 B swizzle granularity), which TMA
-// produces with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; channel groups sit LBO = 4096 B apart, 4-pixel row groups
-// SBO = 512 B apart.  Four tcgen05.mma (M=128, N<=256, K=8 pixels) consume a k-block.  The epilogue warps round
-// both operands to nearest TF32 in shared memory while the tensor core works on earlier stages.
+// each box = 32 rows x 128 B, unswizzled.  wgmma takes 32-bit operands only K-major, so the two consumer warpgroups
+// transpose both operands into 128B-swizzled K-major tiles (one 128-byte row of 32 pixels per channel), rounding them to
+// nearest TF32 on the way, into one of two transposed buffers; the TMA stage is released as soon as it has been read.
+// Four wgmma m64nNk8 per warpgroup (K = 8 pixels) consume a k-block; warpgroup g owns ci rows 64g..64g+63.
 // The pixel range is split across CTAs (split-K); partial tiles go to a workspace and are summed in a fixed order
 // (deterministic), replacing TF's Conv2DBackpropFilter.
 // A conv over a zero-inserted 2x-upsampled input (resnet_ops.py:35-56) is handled through four strided TMA views of dY
@@ -25,9 +24,10 @@ constexpr int WG_MAX_STAGES = 4;
 constexpr int WG_P = 32;                 // pixels per k-block
 constexpr int WG_BOX = WG_P * 128;       // 4 KB: 32 pixel rows x 32 channels fp32
 constexpr int WG_A_BYTES = 4 * WG_BOX;   // 128 input channels
-constexpr int WG_RWARPS = 8;         // warps 2..9: operand rounding, then the epilogue (two warps per TMEM lane quarter)
-constexpr int WG_THREADS = 64 + 32 * WG_RWARPS;
+constexpr int WG_CWARPS = 8;             // two consumer warpgroups
+constexpr int WG_THREADS = 32 * WG_CWARPS + 32;    // + the TMA producer warp
 constexpr int WG_MAX_TAPS = 16;
+constexpr int WG_ACC_COLS = 256;         // mt x bn accumulator columns per CTA
 
 struct WgParams {
   int ntaps;
@@ -36,78 +36,68 @@ struct WgParams {
   int kblocks, kb_per_split;
   int ci_tiles, co_tiles, bn;
   int cin, cout, taps_total;
-  int stages, tmem_cols;                 // pipeline depth chosen so that two CTAs share an SM; TMEM columns = pow2 >= mt*bn
-  int mt;                                // (tap, ci-tile) units per CTA that share one dY tile (mt accumulators in TMEM)
-  int round_a, round_b;                  // round the X / dY tiles to nearest TF32 in shared memory (operand not pre-rounded)
+  int stages;                            // TMA ring depth
+  int mt;                                // (tap, ci-tile) units per CTA that share one dY tile (mt accumulator tiles)
+  int round_a, round_b;                  // round the X / dY tiles to nearest TF32 (operand not pre-rounded)
   float* partial;                        // [split][taps_total][cin][cout]
 };
 
 struct BMaps { CUtensorMap m[4]; };
 
-// MN-major descriptor for 32-bit operands: start>>4 | LBO>>4 (stride between 32-channel groups) | SBO>>4 (stride
-// between 4-pixel row groups) | version 1 | layout SWIZZLE_128B_BASE32B (=1)
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(WG_BOX >> 4) << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;
-  return d;
+// [32 pixels][rows] (unswizzled boxes of 32 channels, box g at g * WG_BOX) -> K-major swizzled [rows][32 pixels]
+__device__ __forceinline__ void wg_transpose(uint32_t dst, uint32_t src, int rows, bool round, int tid) {
+  const int groups = rows / 4;                        // float4 of 4 consecutive channels
+  for (int e = tid; e < groups * WG_P; e += 32 * WG_CWARPS) {
+    const int r = (e % groups) * 4, pix = e / groups;
+    float4 v = lds128(src + (r >> 5) * WG_BOX + pix * 128 + (r & 31) * 4);
+    if (round) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w); }
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r, pix)), "f"(v.x) : "memory");
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 1, pix)), "f"(v.y) : "memory");
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 2, pix)), "f"(v.z) : "memory");
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 3, pix)), "f"(v.w) : "memory");
+  }
 }
 
-__global__ void __launch_bounds__(WG_THREADS, 2)
+template <int BN, int MT>
+__global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMaps tm_dy, const WgParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_bytes = (p.bn / 32) * WG_BOX;
-  const int a_bytes = p.mt * WG_A_BYTES;
-  const int stage_bytes = a_bytes + b_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
-  uint64_t* ready_bar = full_bar + p.stages;
-  uint64_t* empty_bar = ready_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  constexpr int b_bytes = (BN / 32) * WG_BOX;
+  constexpr int a_bytes = MT * WG_A_BYTES;
+  constexpr int stage_bytes = a_bytes + b_bytes;
+  // [stages] TMA ring | [2] transposed K-major operands (same sizes) | barriers
+  uint8_t* tbuf = smem + p.stages * stage_bytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tbuf + 2 * stage_bytes);
+  uint64_t* empty_bar = full_bar + p.stages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work units (tap, ci tile); this CTA owns units [u0, u0 + nu) — they all contract against the same dY tile, which is
-  // fetched from L2 once per k-block for all of them (the kernel is bound by L2->SM bytes per MMA)
+  // fetched from L2 once per k-block for all of them
   int t = blockIdx.x;
   const int co_t = t % p.co_tiles;
-  const int u0 = (t / p.co_tiles) * p.mt;
-  const int nu = min(p.mt, p.ntaps * p.ci_tiles - u0);
+  const int u0 = (t / p.co_tiles) * MT;
+  const int nu = min(MT, p.ntaps * p.ci_tiles - u0);
   const int tap = u0 / p.ci_tiles;               // unit 0's tap: selects the dY view (equal for all units, host-checked)
   const int split = blockIdx.y;
   const int kb0 = split * p.kb_per_split;
   const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
   const int num_kb = kb1 - kb0;                 // >= 1 by construction
-  const int co0 = co_t * p.bn;
+  const int co0 = co_t * BN;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x.m[p.amap[tap]]) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_dy.m[p.bmap[tap]]) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < p.stages; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&ready_bar[s], WG_RWARPS);
-        mbar_init(&empty_bar[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);              // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == WG_CWARPS) {
     if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x.m[p.amap[tap]]) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_dy.m[p.bmap[tap]]) : "memory");
       const CUtensorMap* mb = &tm_dy.m[p.bmap[tap]];
       int stage = 0;
       uint32_t phase = 0;
@@ -129,93 +119,78 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
             tma_load_4d(sa + i * WG_A_BYTES + g * WG_BOX, ma, &full_bar[stage], ci0 + g * 32, w0 + p.off_w[utap],
                         h0 + p.off_h[utap], n0);
         }
-        for (int g = 0; g < p.bn / 32; ++g) tma_load_4d(sb + g * WG_BOX, mb, &full_bar[stage], co0 + g * 32, w0, h0, n0);
+        for (int g = 0; g < BN / 32; ++g) tma_load_4d(sb + g * WG_BOX, mb, &full_bar[stage], co0 + g * 32, w0, h0, n0);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // D=F32, A=B=TF32, both MN-major (bits 15, 16), N>>3, M=128
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(p.bn >> 3) << 17) |
-                           ((uint32_t)(128 >> 4) << 24);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait((p.round_a | p.round_b) ? &ready_bar[stage] : &full_bar[stage], phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-        const uint32_t b_addr = a_addr + a_bytes;
-        for (int i = 0; i < nu; ++i) {
-#pragma unroll
-          for (int k = 0; k < WG_P / 8; ++k)          // 8 pixel rows (1024 B) per MMA
-            umma_tf32(tmem_base + (uint32_t)(i * p.bn), make_desc_mn(a_addr + i * WG_A_BYTES + k * 1024),
-                      make_desc_mn(b_addr + k * 1024), idesc, (kb | k) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (kb == num_kb - 1) umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
-      if (++stage == p.stages) { stage = 0; phase ^= 1; }
-    }
-  } else {
-    const int q = threadIdx.x - 64;
-    if (p.round_a | p.round_b) {
-      int stage = 0;
-      uint32_t phase = 0;
-      // only the operand(s) that are not pre-rounded are swept: [0, a_bytes) is X, [a_bytes, stage_bytes) is dY
-      const int i0 = p.round_a ? 0 : a_bytes / 16;
-      const int n4 = (p.round_b ? stage_bytes : a_bytes) / 16;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t s4 = smem_u32(smem + stage * stage_bytes);
-        // the ranges are multiples of 4 KB (32-pixel boxes of 128 B rows): 256 threads x 16 B per sweep
-#pragma unroll 4
-        for (int i = i0 + q; i < n4; i += 32 * WG_RWARPS) {
-          float4 v = lds128(s4 + i * 16);
-          v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w);
-          sts128(s4 + i * 16, v);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&ready_bar[stage]);
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;           // ci within the tile
-    for (int i = 0; i < nu; ++i) {
-    const int u = u0 + i, utap = u / p.ci_tiles, ci0 = (u % p.ci_tiles) * 128;
-    float* orow = p.partial + (((long long)split * p.taps_total + p.wtap[utap]) * p.cin + ci0 + row) * p.cout + co0;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(i * p.bn);
-    const bool row_ok = ci0 + row < p.cin;       // the last ci tile may hang over Cin (TMA zero-filled those channels)
-    // two warps share a lane quarter: the first takes the lower half of the 32-column chunks, the second the rest
-    const int nchunks = p.bn / 32, csplit = (nchunks + 1) / 2;
-    const int cbeg = (warp - 2) < 4 ? 0 : csplit * 32, cend = (warp - 2) < 4 ? csplit * 32 : p.bn;
-    for (int c0 = cbeg; c0 < cend; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(taddr + (uint32_t)c0, r);       // warp-collective: every lane takes part, stores are predicated
-      if (row_ok) {
-        if (co0 + c0 + 32 <= p.cout && (p.cout & 3) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(orow + c0 + j) =
-                make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-        } else {        // Cout zero-padded to the 32-column tile (e.g. the 24-wide attention projections)
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (co0 + c0 + j < p.cout) orow[c0 + j] = __uint_as_float(r[j]);
-        }
-      }
-    }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
+
+  // ===== consumer warpgroups =====
+  const int wg = warp >> 2;
+  const int tid = threadIdx.x;                   // 0..255
+  float acc[MT][BN / 2];
+#pragma unroll
+  for (int u = 0; u < MT; ++u)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[u][i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t s_addr = smem_u32(smem + stage * stage_bytes);
+    const uint32_t t_addr = smem_u32(tbuf + (kb & 1) * stage_bytes);
+    // both warpgroups' MMAs that read this transposed buffer (k-block kb - 2) retired before the barrier of kb - 1
+    for (int i = 0; i < nu; ++i) wg_transpose(t_addr + i * WG_A_BYTES, s_addr + i * WG_A_BYTES, 128, p.round_a, tid);
+    wg_transpose(t_addr + a_bytes, s_addr + a_bytes, BN, p.round_b, tid);
+    fence_proxy_async();
+    named_bar(1, 32 * WG_CWARPS);
+    if ((tid & 127) == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+    for (int u = 0; u < MT; ++u)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
+    wgmma_fence();
+    // all MT units (one past the end multiplies stale rows that are never stored): one unconditional chain of MMAs
+#pragma unroll
+    for (int u = 0; u < MT; ++u) {
+#pragma unroll
+      for (int k = 0; k < WG_P / 8; ++k)          // 8 pixels (32 B of every row) per MMA
+        wgmma_tf32<BN>(acc[u], make_desc(t_addr + u * WG_A_BYTES + wg * (WG_A_BYTES / 2) + k * 32),
+                       make_desc(t_addr + a_bytes + k * 32));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int u = 0; u < MT; ++u)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+  }
+  // epilogue: rows ci = m, m + 8 of each unit's tile, columns co0 + 8j + 2 (lane % 4) + {0, 1}
+  const int c2 = (lane & 3) * 2;
+  const bool vec2 = (p.cout & 1) == 0;
+#pragma unroll
+  for (int u = 0; u < MT; ++u) {
+    if (u >= nu) continue;
+    const int uu = u0 + u, utap = uu / p.ci_tiles, ci0 = (uu % p.ci_tiles) * 128;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
+      if (ci0 + row >= p.cin) continue;          // the last ci tile may hang over Cin (TMA zero-filled those channels)
+      float* orow = p.partial + (((long long)split * p.taps_total + p.wtap[utap]) * p.cin + ci0 + row) * p.cout + co0;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = j * 8 + c2;
+        if (co0 + c >= p.cout) continue;         // Cout zero-padded to the 32-column tile (e.g. 24-wide projections)
+        if (vec2) {
+          *reinterpret_cast<float2*>(orow + c) = make_float2(acc[u][4 * j + 2 * h], acc[u][4 * j + 2 * h + 1]);
+        } else {
+          orow[c] = acc[u][4 * j + 2 * h];
+          if (co0 + c + 1 < p.cout) orow[c + 1] = acc[u][4 * j + 2 * h + 1];
+        }
+      }
+    }
   }
 }
 
@@ -246,6 +221,37 @@ int pick_bn(int ncols) {
   if (ncols % 192 == 0) return 192;
   if (ncols % 128 == 0) return 128;
   return 0;
+}
+
+// TMA ring depth for a shared-memory budget (ring + the two transposed buffers); returns the dynamic smem size
+size_t wg_smem(size_t stage_bytes, size_t budget, int* stages) {
+  long long s = (long long)(budget / stage_bytes) - 2;
+  if (s > WG_MAX_STAGES) s = WG_MAX_STAGES;
+  if (s < 2) s = 2;
+  *stages = (int)s;
+  return (size_t)(s + 2) * stage_bytes + 1024 + 256;
+}
+
+template <int BN, int MT>
+int wg_launch_t(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BMaps& tm_dy, const WgParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    CGAN_CUDA(ctx, cudaFuncSetAttribute(wgrad_tc_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  wgrad_tc_kernel<BN, MT><<<grid, WG_THREADS, smem, ctx->stream>>>(tm_x, tm_dy, p);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+// one instantiation per (bn, mt): the accumulator fragment is sized at compile time
+int wg_launch(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BMaps& tm_dy, const WgParams& p) {
+#define WG_CASE(BN, MT) \
+  if (p.bn == BN && p.mt == MT) return wg_launch_t<BN, MT>(ctx, grid, smem, tm_x, tm_dy, p);
+  WG_CASE(32, 1) WG_CASE(64, 1) WG_CASE(96, 1) WG_CASE(128, 1) WG_CASE(160, 1) WG_CASE(192, 1) WG_CASE(224, 1)
+  WG_CASE(256, 1) WG_CASE(32, 2) WG_CASE(64, 2) WG_CASE(96, 2) WG_CASE(128, 2)
+#undef WG_CASE
+  return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: no kernel for this column tile%s", "cgan_wgrad_tc");
 }
 
 }  // namespace
@@ -309,11 +315,13 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const 
   const int units = p.ci_tiles * nt;
   bool same_b = true;
   for (int i = 1; i < nt; ++i) same_b = same_b && p.bmap[i] == p.bmap[0];
-  p.mt = (ctx->tc_mt_max >= 2 && same_b && units >= 2) ? 2 : 1;
-  const bool two_ctas = p.mt * p.bn <= 256;      // TMEM: mt*bn accumulator columns per CTA, 512 per SM
+  p.mt = (ctx->tc_mt_max >= 2 && same_b && units >= 2 && 2 * p.bn <= WG_ACC_COLS) ? 2 : 1;
+  const size_t stage_bytes = (size_t)p.mt * WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
+  const bool two_ctas = wg_smem(stage_bytes, 110 * 1024, &p.stages) <= 113 * 1024;
   long long tiles = (long long)p.co_tiles * ((units + p.mt - 1) / p.mt);
-  // one wave of CTAs, rounded DOWN so the grid never spills a few CTAs into an extra wave
-  int splits = (int)(((two_ctas ? 2ll : 1ll) * ctx->num_sms) / tiles);
+  // two CTAs per SM in total (two waves when only one fits), rounded DOWN so the grid never spills a few CTAs into an
+  // extra wave; the pixel chain each fp32 accumulator sums stays as short as with two resident CTAs per SM
+  int splits = (int)((2ll * ctx->num_sms) / tiles);
   int max_splits = p.kblocks / 8 > 0 ? p.kblocks / 8 : 1;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
@@ -339,10 +347,10 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const 
       int a = v >> 1, b = v & 1;
       ok = make_act_map(&tm_x.m[v], x + ((long long)a * d->w + b) * d->cin, d->cin, gw, gh, d->n, 2ll * d->cin,
                         2ll * d->w * d->cin, (long long)d->h * d->w * d->cin, p.bw, p.bh, p.bni,
-                        CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+                        CU_TENSOR_MAP_SWIZZLE_NONE);
     } else {
       ok = make_act_map(&tm_x.m[v], x, d->cin, d->w, d->h, d->n, d->cin, (long long)d->w * d->cin,
-                        (long long)d->h * d->w * d->cin, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+                        (long long)d->h * d->w * d->cin, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE);
     }
     if (!ok) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(x) failed%s", "cgan_wgrad_tc");
   }
@@ -350,30 +358,18 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const 
     bool ok;
     if (!d->upsample) {
       ok = make_act_map(&tm_dy.m[v], dy, d->cout, gw, gh, d->n, d->cout, (long long)d->ow * d->cout,
-                        (long long)d->oh * d->ow * d->cout, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+                        (long long)d->oh * d->ow * d->cout, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE);
     } else {
       int a = v >> 1, b = v & 1;
       ok = make_act_map(&tm_dy.m[v], dy + ((long long)a * d->ow + b) * d->cout, d->cout, d->w, d->h, d->n, 2ll * d->cout,
                         2ll * d->ow * d->cout, (long long)d->oh * d->ow * d->cout, p.bw, p.bh, p.bni,
-                        CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+                        CU_TENSOR_MAP_SWIZZLE_NONE);
     }
     if (!ok) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(dy) failed%s", "cgan_wgrad_tc");
   }
-  const size_t stage_bytes = (size_t)p.mt * WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
-  p.stages = (int)(((two_ctas ? 110 : 220) * 1024) / stage_bytes);
-  if (p.stages > WG_MAX_STAGES) p.stages = WG_MAX_STAGES;
-  if (p.stages < 2) p.stages = 2;
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.mt * p.bn) p.tmem_cols *= 2;
-  size_t smem = (size_t)p.stages * stage_bytes + 1024 + 256;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CGAN_CUDA(ctx, cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  dim3 grid((unsigned)tiles, (unsigned)splits);
-  wgrad_tc_kernel<<<grid, WG_THREADS, smem, ctx->stream>>>(tm_x, tm_dy, p);
-  CGAN_LAUNCHED(ctx);
+  const size_t smem = wg_smem(stage_bytes, two_ctas ? 110 * 1024 : 220 * 1024, &p.stages);
+  int rc = wg_launch(ctx, dim3((unsigned)tiles, (unsigned)splits), smem, tm_x, tm_dy, p);
+  if (rc) return rc;
   if (splits > 1) {
     wg_reduce_kernel<<<cdiv(wn, 256), 256, 0, ctx->stream>>>(dw, partial, wn, splits);
     CGAN_LAUNCHED(ctx);
@@ -407,26 +403,13 @@ int cgan_wgrad_tc_batched(cgan_ctx* ctx, const float* a, const float* b, float* 
   memset(&tm_dy, 0, sizeof(tm_dy));
   for (int v = 0; v < 4; ++v) {
     if (!make_act_map(&tm_x.m[v], a, k1, w, h, batch, k1, (long long)w * k1, (long long)h * w * k1, p.bw, p.bh, p.bni,
-                      CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) ||
+                      CU_TENSOR_MAP_SWIZZLE_NONE) ||
         !make_act_map(&tm_dy.m[v], b, k2, w, h, batch, k2, (long long)w * k2, (long long)h * w * k2, p.bw, p.bh, p.bni,
-                      CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
+                      CU_TENSOR_MAP_SWIZZLE_NONE))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed%s", "cgan_wgrad_tc_batched");
   }
   const size_t stage_bytes = WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
-  p.stages = (int)((110 * 1024) / stage_bytes);
-  if (p.stages > WG_MAX_STAGES) p.stages = WG_MAX_STAGES;
-  if (p.stages < 2) p.stages = 2;
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.bn) p.tmem_cols *= 2;
-  size_t smem = (size_t)p.stages * stage_bytes + 1024 + 256;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CGAN_CUDA(ctx, cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
+  const size_t smem = wg_smem(stage_bytes, 110 * 1024, &p.stages);
   if (batch > 65535) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: batch exceeds grid.y%s", "cgan_wgrad_tc_batched");
-  dim3 grid((unsigned)(p.ci_tiles * p.co_tiles), (unsigned)batch);
-  wgrad_tc_kernel<<<grid, WG_THREADS, smem, ctx->stream>>>(tm_x, tm_dy, p);
-  CGAN_LAUNCHED(ctx);
-  return CGAN_OK;
+  return wg_launch(ctx, dim3((unsigned)(p.ci_tiles * p.co_tiles), (unsigned)batch), smem, tm_x, tm_dy, p);
 }

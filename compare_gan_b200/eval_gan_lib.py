@@ -75,7 +75,7 @@ class _EvalBatchGraph(object):
   evaluates in batches of 64 (eval_gan_lib.py:113); in inference mode every sample is independent of its batch mates
   (moving averages / accumulators, no batch statistics), so running `fuse` consecutive batches as one device batch gives
   bit-identical features while the 17x17 and 8x8 Inception stages get `fuse` times as many pixel tiles per launch (at 64
-  images they expose 145 / 32 tiles to 148 SMs).  The z / label stream is still drawn batch by batch in the same order."""
+  images they expose 145 / 32 tiles to 132 SMs).  The z / label stream is still drawn batch by batch in the same order."""
 
   def __init__(self, gan, batch_size, acc, fuse=1):
     dev = K._RT["device"]

@@ -1,6 +1,6 @@
 """Public names of the weight initialisers and architectures that gin files and `ModularGAN` refer to (the string values
 are the reference's, gans/consts.py:28-40, because `options.architecture = "resnet_cifar_arch"` etc. must keep working).
-`IMPLEMENTED_ARCHITECTURES` are the ones the B200 engine builds; asking for any other raises NotImplementedError in
+`IMPLEMENTED_ARCHITECTURES` are the ones the H100 engine builds; asking for any other raises NotImplementedError in
 `ModularGAN` exactly as an unknown name does in the reference (modular_gan.py:184-187)."""
 
 # weights.initializer values -> NORMAL_INIT, TRUNCATED_INIT, ORTHOGONAL_INIT

@@ -28,7 +28,7 @@ def _objective(kind, logits_first):
   def run(d_real, d_fake, d_real_logits, d_fake_logits):
     check_dimensions(d_real, d_fake, d_real_logits, d_fake_logits)
     if d_real_logits is None or d_fake_logits is None:
-      raise ValueError("The B200 loss kernel works from logits; pass d_real_logits and d_fake_logits.")
+      raise ValueError("The loss kernel works from logits; pass d_real_logits and d_fake_logits.")
     return K.gan_losses(kind, d_real_logits, d_fake_logits)     # sigmoid(logits) is recomputed inside the kernel
 
   if logits_first:

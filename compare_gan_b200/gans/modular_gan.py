@@ -1,4 +1,4 @@
-"""ModularGAN: the training step (reference gans/modular_gan.py:56-670) on one B200 per process.
+"""ModularGAN: the training step (reference gans/modular_gan.py:56-670) on one H100 per process.
 
 What TF did with a static graph + TPUEstimator is done here with:
   * an eager "cycle" (disc_iters D-updates + 1 G-update, the unrolled/TPU semantics of
@@ -73,7 +73,7 @@ class ModularGAN(AbstractGAN):
       raise ValueError("Option 'conditional' selected but dataset {} does not have labels".format(
           self._dataset.name))
     self._conditional = conditional
-    # 0: exact fp32 contractions (parity mode); 1: tcgen05 kind::tf32 tensor-core convolutions (RN-rounded operands)
+    # 0: exact fp32 contractions (parity mode); 1: wgmma TF32 tensor-core convolutions (RN-rounded operands)
     self._math_mode = math_mode
     self._architecture = parameters["architecture"]
     self._z_dim = parameters["z_dim"]

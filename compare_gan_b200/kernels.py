@@ -1,4 +1,4 @@
-"""Taped device ops: each function launches sm_100a kernels through the C-ABI (include/cgan_b200.h)
+"""Taped device ops: each function launches sm_90a kernels through the C-ABI (include/cgan_b200.h)
 and records its vector-Jacobian product on the tape (tape.py).  The vjps of the ops a discriminator
 without normalisation is made of (convolutions, matmul, bias, (leaky) ReLU, pools, reshapes, adds) are
 written with the same taped ops, so second-order differentiation (WGAN-GP, gans/penalty_lib.py:59-82)
@@ -6,7 +6,7 @@ works by construction for them.  The vjps of batch norm, softmax and spectral no
 weight launch raw kernels: differentiating THROUGH them (a gradient penalty on a discriminator with
 BN / attention) raises NotImplementedError instead of silently dropping the second-order terms.
 
-These are the B200 stand-ins for the TF library calls the reference's ops library makes
+These are the H100 stand-ins for the TF library calls the reference's ops library makes
 (arch_ops.py / resnet_ops.py / loss_lib.py / penalty_lib.py); file:line citations sit on each op.
 """
 import ctypes
@@ -543,7 +543,7 @@ def round_tf32(x):
 
 
 def attention_shape_ok(bsz, lq, lk, dk, dv):
-  """Do the fused tcgen05 attention kernels take this shape in the current math mode?"""
+  """Do the fused wgmma attention kernels take this shape in the current math mode?"""
   return bool(tf32_on() and lib().attention_supported(bsz, lq, lk, dk, dv))
 
 
@@ -554,8 +554,8 @@ def attention_fused_ok(theta, phi, g):
 
 def attention(theta, phi, g):
   """softmax(theta phi^T) g per image — tf.matmul(theta, phi, transpose_b=True) -> tf.nn.softmax -> tf.matmul(attn, g)
-  (arch_ops.py:744-753).  In math_mode 1, for shapes the fused tcgen05 kernels take (csrc/attn_tc.cu: BigGAN's 4096 x 1024
-  scores at 24 / 12 key channels), ONE kernel per direction keeps the scores in TMEM / shared memory; otherwise the three
+  (arch_ops.py:744-753).  In math_mode 1, for shapes the fused wgmma kernels take (csrc/attn_tc.cu: BigGAN's 4096 x 1024
+  scores at 24 / 12 key channels), ONE kernel per direction keeps the scores in registers; otherwise the three
   ops are composed as the reference writes them."""
   if not attention_fused_ok(theta, phi, g):
     return bmm(softmax(bmm(theta, phi, False, True)), g)
@@ -1090,7 +1090,7 @@ def gp_penalty(g):
 
 
 def set_math_mode(mode):
-  """0: exact fp32 SIMT contractions; 1: tcgen05 kind::tf32 tensor-core convolutions where the shape allows
-  (operands rounded to nearest TF32, fp32 accumulation in TMEM)."""
+  """0: exact fp32 SIMT contractions; 1: wgmma TF32 tensor-core convolutions where the shape allows
+  (operands rounded to nearest TF32, fp32 accumulation)."""
   _call("ctx_set_math_mode", int(mode))
   _RT["math_mode"] = int(mode)

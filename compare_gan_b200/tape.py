@@ -2,7 +2,7 @@
 
 TensorFlow's graph autodiff (tf.gradients, used by optimizer.minimize at
 gans/modular_gan.py:478-497 and by the gradient penalties at gans/penalty_lib.py:78) is
-replaced by a small tape: every op in `kernels.py` launches sm_100a kernels through the C-ABI
+replaced by a small tape: every op in `kernels.py` launches sm_90a kernels through the C-ABI
 and records a vector-Jacobian closure that is itself written in terms of those ops, so the
 WGAN-GP second backward needs no special casing.  PyTorch is used for device memory only
 (`torch.empty`); no torch op, no torch.autograd, on this path.  The Python overhead disappears

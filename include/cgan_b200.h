@@ -1,10 +1,10 @@
-/* cgan_b200.h — C-ABI of the B200 (sm_100a) GAN-step / FID engine.
+/* cgan_b200.h — C-ABI of the H100 (sm_90a) GAN-step / FID engine.
  *
  * The reference (google/compare_gan) has no FFI: its seam is the Python ops library
  * (compare_gan/architectures/arch_ops.py, resnet_ops.py, gans/loss_lib.py, gans/penalty_lib.py,
  * tf.train.AdamOptimizer, tfgan FID).  Each entry point below replaces the TF library kernel(s)
  * behind one of those call sites; the citation after each declaration is the reference
- * file:line it stands in for (paths relative to /root/reference/compare_gan/).
+ * file:line it stands in for (paths relative to the reference's compare_gan/ package).
  *
  * Conventions
  *  - plain pointers and sizes only; every pointer is a DEVICE pointer unless named host_*.
@@ -35,27 +35,30 @@ int cgan_ctx_create(cgan_ctx** out, int device);
 int cgan_ctx_destroy(cgan_ctx* ctx);
 int cgan_ctx_set_stream(cgan_ctx* ctx, void* cuda_stream);          /* cudaStream_t */
 int cgan_ctx_reserve_workspace(cgan_ctx* ctx, size_t bytes);        /* pre-size (never during capture) */
-/* 0: exact fp32 SIMT contraction; 1: tcgen05 kind::tf32 tensor-core path where the shape allows. */
+/* 0: exact fp32 SIMT contraction; 1: wgmma TF32 tensor-core path where the shape allows. */
 int cgan_ctx_set_math_mode(cgan_ctx* ctx, int mode);
 const char* cgan_last_error(cgan_ctx* ctx);
 /* number of kernels this context has launched since creation (bench.py's gpu_launches). */
 int64_t cgan_launch_count(cgan_ctx* ctx);
 /* Tuning knobs and introspection (tests compare kernel variants bit for bit and ask which path a contraction took).
- *   CGAN_OPT_TC_MT      (set/get) max pixel tiles (conv) / work units (filter gradient) per tcgen05 CTA: 1 or 2.
- *   CGAN_OPT_TC_HALO    (set/get) 3x3 stride-1 tcgen05 convolutions fetch one (rows+2)-row activation box per kernel column
- *                       instead of one box per tap: 0 never, 1 where it measured faster (operand rounded in the kernel,
- *                       >= 256 output channels; default), 2 wherever the geometry allows.
- *   CGAN_OPT_TC_PAIR    (set/get) 1: tcgen05 convolutions run as CTA pairs (cta_group::2, M = 256) sharing each weight tile.
- *   CGAN_OPT_TC_EPI     (set/get) 1 (default): the tcgen05 convolution epilogue transposes each 32 x 32 accumulator chunk through
- *                       shared memory so that stores (and the fused residual / mask reads) cover whole 128-byte lines;
- *                       0: every thread stores its own row (the round-1 epilogue; results are bit-identical).
+ *   CGAN_OPT_TC_MT      (set/get) max pixel tiles (conv) / work units (filter gradient) per tensor-core CTA: 1 or 2
+ *                       (2 only where the accumulators of both fit the registers: column tiles <= 128 wide).
+ *   CGAN_OPT_TC_HALO    (set/get) 3x3 stride-1 tensor-core convolutions fetch one (rows+2)-row activation box per kernel
+ *                       column instead of one box per tap: 0 never, 1 where the operand is rounded in the kernel and there
+ *                       are >= 256 output channels (default), 2 wherever the geometry allows.
+ *   CGAN_OPT_TC_PAIR    (set/get) 1: the per-tap tensor-core convolutions run as two-CTA clusters that share each weight
+ *                       tile through TMA multicast (same products in the same order); 0 (default): single CTAs, which
+ *                       measured faster on an H100 (3x3 256->256 and 128->128 convs at 32x32).
+ *   CGAN_OPT_TC_EPI     (set/get) accepted and reported; the epilogue stores straight from the accumulator fragments
+ *                       (a lane quad covers 32 contiguous bytes of a row) for every value.
  *   CGAN_OPT_TC_THIN    (set/get) 1 (default): in math_mode 1 the image-side convolutions (<= 4 input or <= 4 output channels,
  *                       kh*kw*channels <= 32: every discriminator's first and every generator's last convolution, Inception's
- *                       stem) run as ONE 32-wide GEMM on the tcgen05 kernels over a [pixels, 32] patch tensor (csrc/thin_tc.cu),
+ *                       stem) run as ONE 32-wide GEMM on the tensor-core kernels over a [pixels, 32] patch tensor (csrc/thin_tc.cu),
  *                       TF32 operands like every other tensor-core contraction; 0: the exact-fp32 streaming kernels (thin.cu).
  *   CGAN_OPT_LAST_PATH  (get) CGAN_PATH_* taken by the most recent conv2d_fwd / dgrad / wgrad / gemm_batched call. */
 enum { CGAN_OPT_TC_MT = 1, CGAN_OPT_LAST_PATH = 2, CGAN_OPT_TC_HALO = 3, CGAN_OPT_TC_PAIR = 4, CGAN_OPT_TC_EPI = 5,
        CGAN_OPT_TC_THIN = 6 };
+/* CGAN_PATH_TCGEN05_TF32 keeps its name for ABI compatibility: the TF32 tensor-core (wgmma) path. */
 enum { CGAN_PATH_SIMT_FP32 = 0, CGAN_PATH_TCGEN05_TF32 = 1, CGAN_PATH_THIN_FP32 = 2 };
 int cgan_ctx_set_option(cgan_ctx* ctx, int key, int64_t value);
 int cgan_ctx_get_option(cgan_ctx* ctx, int key, int64_t* host_value);
@@ -140,8 +143,8 @@ int cgan_gemm_batched(cgan_ctx*, int trans_a, int trans_b, int m, int n, int k, 
 
 /* ---- fused self-attention (non_local_block, arch_ops.py:734-753) --------------------------------------------------
  * out[i] = softmax(q[i] k[i]^T) v[i] per image i: q = theta [batch, lq, dk], k = phi [batch, lk, dk], v = g [batch, lk, dv],
- * out [batch, lq, dv] — tf.matmul(theta, phi, transpose_b=True) -> tf.nn.softmax -> tf.matmul(attn, g) in ONE tcgen05
- * kernel: the [lq, lk] scores live in TMEM / shared memory only (csrc/attn_tc.cu).  lse [batch, lq] receives the
+ * out [batch, lq, dv] — tf.matmul(theta, phi, transpose_b=True) -> tf.nn.softmax -> tf.matmul(attn, g) in ONE wgmma
+ * kernel: the [lq, lk] scores live in registers only (csrc/attn_tc.cu).  lse [batch, lq] receives the
  * log-sum-exp of every score row; the backward recomputes the probabilities from it.  Operands are consumed as TF32:
  * pass tensors that already hold TF32-representable values (cgan_round_tf32, or a producer's ROUND_OUT epilogue).
  * cgan_attention_supported returns 1 when the fused kernels accept the shape in the current math mode (math_mode 1,

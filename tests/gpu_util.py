@@ -215,7 +215,8 @@ def compare_states(eng, orc, lr, updates, frac=0.35, skip=(), state_tol=2e-3):
         continue   # noise-dominated gradient (zero in exact arithmetic)
       rms = float(np.sqrt(np.mean((a.astype(np.float64) - b) ** 2)))
       lim = frac * lr[k.split("/")[0]] * updates[k.split("/")[0]]
-      worst = max(worst, (rms / lim, k))
+      if rms / lim >= worst[0]:
+        worst = (rms / lim, k)
       assert rms <= lim, "%s: rms weight error %.3e > %.3e" % (k, rms, lim)
     else:
       e = rel_err(a, b)

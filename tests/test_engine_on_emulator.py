@@ -81,7 +81,7 @@ def _kernel_test_cases():
 def test_emulator_conforms_to_the_kernel_parity_suite():
   """The per-op parity tests define what each C-ABI entry must compute (against the oracle).  Running them against the
   emulator shows that the emulator — on which the host-code tests above rest — honours the same contract.  Only the
-  assertions that the tcgen05 path was TAKEN (launch counts of the tensor-core kernels) are specific to the real
+  assertions that the tensor-core path was TAKEN (launch counts of the tensor-core kernels) are specific to the real
   library and are skipped."""
   import inspect
   from compare_gan_b200 import kernels as K

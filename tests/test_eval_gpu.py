@@ -87,7 +87,7 @@ def test_eval_fid_is_kid_against_oracle(K):
 
 def test_inception_v3_features_tf32(K):
   """math_mode 1: the stride-1 SAME convolutions of Inception (35x35 / 17x17 / 8x8 maps, 1x7 / 7x1 / 5x5 kernels, 48/80-
-  channel inputs) run on tcgen05 through border-overhanging 128-pixel boxes and zero-padded K; pool_3 within 2e-3."""
+  channel inputs) run on the tensor cores through border-overhanging 128-pixel boxes and zero-padded K; pool_3 within 2e-3."""
   from compare_gan_b200 import inception
   w = inception.synthetic_weights(0)
   rng = np.random.RandomState(2)

@@ -200,7 +200,7 @@ def eng_launches():
 
 
 def test_resnet_cifar_cycle_tf32_tensor_cores():
-  """math_mode 1: the same cycle with the convolutions on tcgen05 (TF32 operands rounded to nearest, fp32 TMEM
+  """math_mode 1: the same cycle with the convolutions on wgmma (TF32 operands rounded to nearest, fp32
   accumulation).  north_star tolerance: per-tensor activations within 1e-3 rel; gradients checked at 1e-2 (TF32 noise
   passes through ~15 layers and BatchNorm's cancellation), losses at 1e-3."""
   from compare_gan_b200 import kernels as K

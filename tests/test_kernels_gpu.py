@@ -78,8 +78,8 @@ def test_conv2d_fwd_dgrad_wgrad(K, n, h, cin, cout, k, stride, up):
     (0, 3, 10, 3, 96, 1, False),        # pointwise stream kernel (residual fused in the kernel)
     (0, 2, 12, 3, 32, 3, False),        # 3x3 image-side kernel + post pass
     (0, 2, 8, 16, 24, 3, False),        # exact fp32 SIMT + post pass
-    (1, 4, 16, 64, 64, 3, False),       # tcgen05 epilogue
-    (1, 4, 8, 64, 96, 3, True),         # tcgen05, sub-pixel phases
+    (1, 4, 16, 64, 64, 3, False),       # tensor-core epilogue
+    (1, 4, 8, 64, 96, 3, True),         # tensor cores, sub-pixel phases
     (1, 4, 8, 64, 64, 1, True),         # 1x1 over the zero-inserted input (phase 0 + bias phases + post pass)
 ])
 def test_conv2d_fused_epilogue(K, mode, n, h, cin, cout, k, up):
@@ -415,7 +415,7 @@ def test_cov_accumulate_and_fid(K):
 
 
 TC_CASES = [
-    # n, h, cin, cout, k, upsample      (shapes the tcgen05 path accepts: cin%32==0, cout%32==0, 128-pixel boxes)
+    # n, h, cin, cout, k, upsample      (shapes the tensor-core path accepts: cin%32==0, cout%32==0, 128-pixel boxes)
     (2, 8, 32, 32, 3, False),
     (2, 8, 64, 128, 3, False),
     (8, 4, 64, 64, 3, False),
@@ -439,14 +439,14 @@ TC_CASES = [
     (2, 17, 128, 192, 7, False),   # 17x17 map; square 7x7 here (49 taps) falls back to the gather-GEMM
     (5, 8, 80, 96, 3, False),      # 8x8 maps, odd batch: the last tile hangs over the batch
     (1, 147, 32, 64, 3, False),    # 147-wide rows split into two 74-pixel boxes
-    (8, 4, 32, 64, 1, True),       # 1x1 over a zero-inserted input: phase (0,0) on tcgen05 + bias-only phases
+    (8, 4, 32, 64, 1, True),       # 1x1 over a zero-inserted input: phase (0,0) on the tensor cores + bias-only phases
     (2, 16, 192, 96, 1, True),
 ]
 
 
 @pytest.mark.parametrize("n,h,cin,cout,k", [(2, 16, 64, 128, 4), (8, 8, 128, 256, 4), (2, 32, 64, 64, 3), (1, 64, 128, 128, 4)])
 def test_conv2d_stride2_tcgen05(K, n, h, cin, cout, k):
-  """Stride-2 convs (SNDCGAN D 4x4 s2, and its generator's transposed convs = their input gradient) on tcgen05 through
+  """Stride-2 convs (SNDCGAN D 4x4 s2, and its generator's transposed convs = their input gradient) on the tensor cores through
   the four parity-phase TMA views."""
   rng = np.random.RandomState(n * 100 + h + cin + k)
   x = rng.randn(n, h, h, cin).astype(np.float32)
@@ -461,7 +461,7 @@ def test_conv2d_stride2_tcgen05(K, n, h, cin, cout, k):
     xd, wd, bd = dev(K, x, True), dev(K, w, True), dev(K, b, True)
     n0 = K.lib().launch_count()
     y = K.conv2d(xd, wd, bd, stride=2)
-    assert K.lib().launch_count() - n0 == 2, "expected weight prep + one tcgen05 launch"
+    assert K.lib().launch_count() - n0 == 2, "expected weight prep + one tensor-core launch"
     assert_close(y.cpu(), ref.detach().numpy(), 1e-3, "s2 fwd")
     gx, gw = tape_grads(K, y, gy, [xd, wd])
     assert_close(gx.cpu(), xt.grad.numpy(), 1e-3, "s2 dgrad")
@@ -472,7 +472,7 @@ def test_conv2d_stride2_tcgen05(K, n, h, cin, cout, k):
 
 @pytest.mark.parametrize("n,h,cin,cout,k,up", TC_CASES)
 def test_conv2d_tcgen05_tf32(K, n, h, cin, cout, k, up):
-  """math_mode 1: tcgen05 kind::tf32 implicit GEMM (TMA-staged, TMEM accumulators) vs the fp32 oracle.
+  """math_mode 1: wgmma TF32 implicit GEMM (TMA-staged, register accumulators) vs the fp32 oracle.
   Tolerance 1e-3 rel-L2 (north_star's per-tensor bound); expected ~3e-4 for RN-rounded TF32 operands."""
   rng = np.random.RandomState(hash((n, h, cin, cout, k, up)) % 2**31)
   x = rng.randn(n, h, h, cin).astype(np.float32)
@@ -490,13 +490,13 @@ def test_conv2d_tcgen05_tf32(K, n, h, cin, cout, k, up):
     y = K.conv2d(xd, wd, bd, stride=1, upsample=up)
     launched = K.lib().launch_count() - n0
     if k == 1 and up:
-      assert launched == 3, "1x1 up-sampling conv: weight prep + one tcgen05 phase + bias fill, got %d" % launched
+      assert launched == 3, "1x1 up-sampling conv: weight prep + one tensor-core phase + bias fill, got %d" % launched
     elif min(cin, cout) <= 4 and not up:
-      # image-side layer (csrc/thin_tc.cu): filter re-layout + weight prep + ONE 32-wide tcgen05 GEMM + the shift-add pass
-      assert launched == 4, "expected the patch-tensor tcgen05 path (4 launches), got %d" % launched
+      # image-side layer (csrc/thin_tc.cu): filter re-layout + weight prep + ONE 32-wide tensor-core GEMM + the shift-add pass
+      assert launched == 4, "expected the patch-tensor tensor-core path (4 launches), got %d" % launched
     elif k * k <= 32:
       # (the four sub-pixel phases of a convolution over a zero-inserted input share one weight preparation and ONE launch)
-      assert launched == 2, "expected the tcgen05 path (weight prep + one launch), got %d launches" % launched
+      assert launched == 2, "expected the tensor-core path (weight prep + one launch), got %d launches" % launched
     assert_close(y.cpu(), ref.detach().numpy(), 1e-3, "tc conv fwd")
     gx, gw = tape_grads(K, y, gy, [xd, wd])
     assert_close(gx.cpu(), xt.grad.numpy(), 1e-3, "tc conv dgrad")
@@ -511,7 +511,7 @@ def test_conv2d_tcgen05_tf32(K, n, h, cin, cout, k, up):
 
 @pytest.mark.parametrize("n,h,cin,cout,k", [(2, 35, 64, 96, 3), (1, 71, 80, 192, 3), (3, 8, 32, 64, 5)])
 def test_conv2d_valid_padding_tcgen05(K, n, h, cin, cout, k):
-  """VALID (unpadded) stride-1 convolutions (Inception stem) on tcgen05: the tile grid is the smaller output extent."""
+  """VALID (unpadded) stride-1 convolutions (Inception stem) on the tensor cores: the tile grid is the smaller output extent."""
   import torch.nn.functional as F
   rng = np.random.RandomState(h + cin)
   x = rng.randn(n, h, h, cin).astype(np.float32)
@@ -555,7 +555,7 @@ def test_conv2d_stride2_any_size_tcgen05(K, n, h, cin, cout, k, pad):
   finally:
     K.set_math_mode(0)
   if cin % 4 == 0:
-    assert launched == 2, "expected the tcgen05 path"
+    assert launched == 2, "expected the tensor-core path"
   assert y.shape == tuple(ref.shape)
   assert_close(y.cpu(), torch.relu(ref).numpy(), 1e-3, "stride-2 %s conv" % pad)
 
@@ -578,7 +578,7 @@ def test_softmax_rows(K, rows, cols):
 @pytest.mark.parametrize("bsz,m,kv,ca,cg", [(3, 1024, 256, 24, 96), (2, 4096, 1024, 12, 48), (5, 256, 64, 32, 64)])
 def test_tc_batched_matmul_attention(K, bsz, m, kv, ca, cg):
   """math_mode 1: the attention products of the non-local block (arch_ops.py:744, 753) and all four of their
-  gradients run as per-image GEMMs on tcgen05: nt / nn through the conv kernel (per-image weight slice), tn through
+  gradients run as per-image GEMMs on the tensor cores: nt / nn through the conv kernel (per-image weight slice), tn through
   the filter-gradient kernel (one image per CTA row)."""
   rng = np.random.RandomState(m + kv)
   theta = rng.randn(bsz, m, ca).astype(np.float32)
@@ -595,7 +595,7 @@ def test_tc_batched_matmul_attention(K, bsz, m, kv, ca, cg):
     n0 = K.lib().launch_count()
     s = K.affine(K.bmm(td, pd, False, True), 1.0 / np.sqrt(ca))
     y = K.bmm(s, gd)
-    assert K.lib().launch_count() - n0 == 5, "expected 2 x (operand prep + tcgen05 launch) + scale"
+    assert K.lib().launch_count() - n0 == 5, "expected 2 x (operand prep + tensor-core launch) + scale"
     assert_close(y.cpu(), ref.detach().numpy(), 2e-3, "attn fwd")
     n0 = K.lib().launch_count()
     gth, gph, gg = tape_grads(K, y, gy, [td, pd, gd])
@@ -648,7 +648,7 @@ def _rna_tf32(a):
                                               (2, 4096, 1024, 12, 48), (1, 128, 128, 32, 128), (2, 256, 128, 4, 16)])
 def test_tc_fused_attention(K, bsz, lq, lk, dk, dv):
   """math_mode 1: softmax(theta phi^T) g of the non-local block (arch_ops.py:744-753) and its three gradients in the fused
-  tcgen05 kernels (csrc/attn_tc.cu) — scores only in TMEM / shared memory.  Checked (a) against the float64 evaluation on the
+  wgmma kernels (csrc/attn_tc.cu) — scores only in registers.  Checked (a) against the float64 evaluation on the
   SAME TF32-rounded operands (what remains is the TF32 rounding of the probabilities and fp32 accumulation: <= 5e-4), (b) against
   the reference's own composition tf.matmul -> tf.nn.softmax -> tf.matmul in fp32 on the unrounded operands at north_star's
   1e-3, and (c) against the engine's composed path (three launches per direction) in exact-fp32 mode."""
@@ -720,7 +720,7 @@ THIN_TC_CASES = [
 
 @pytest.mark.parametrize("n,h,cin,cout,k,stride,pad", THIN_TC_CASES)
 def test_thin_convolutions_on_tensor_cores(K, n, h, cin, cout, k, stride, pad):
-  """math_mode 1: convolutions with <= 4 input or output channels run as one 32-wide tcgen05 GEMM over a [pixels, 32] patch
+  """math_mode 1: convolutions with <= 4 input or output channels run as one 32-wide tensor-core GEMM over a [pixels, 32] patch
   tensor (csrc/thin_tc.cu) — forward, input gradient and filter gradient against the fp32 oracle at north_star's 1e-3, and
   against the exact-fp32 streaming kernels they replace (CGAN_OPT_TC_THIN = 0)."""
   from compare_gan_b200 import _lib

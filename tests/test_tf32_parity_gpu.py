@@ -1,4 +1,4 @@
-"""Parity of the BENCHMARKED path: math_mode 1 (tcgen05 kind::tf32 convolutions, TF32-rounded operands, fp32 accumulate).
+"""Parity of the BENCHMARKED path: math_mode 1 (wgmma TF32 convolutions, TF32-rounded operands, fp32 accumulate).
 
 Two yard-sticks, both CPU oracles (oracle/):
   * the fp32 restatement of the reference — what north_star's tolerance (per-tensor activations within 1e-3 rel) is
@@ -48,7 +48,7 @@ BASELINE_SHAPES = [
 @pytest.mark.parametrize("name,n,h,cin,cout,k,up", BASELINE_SHAPES)
 def test_tcgen05_baseline_shapes_mt2_bit_equals_mt1_and_matches_oracle(K, name, n, h, cin, cout, k, up):
   """The conv shapes bench.py runs (batch 256 per GPU): forward, input gradient and filter gradient with two pixel tiles
-  per CTA (mt = 2, taken when there are >= 4 x 148 tiles) are BIT-identical to the one-tile variant (filter gradient: 5e-5,
+  per CTA (mt = 2, taken when there are >= 4 tiles per SM) are BIT-identical to the one-tile variant (filter gradient: 5e-5,
 its deterministic split-K grouping follows the CTA count), and match the fp32
   oracle within 1e-3 rel-L2 (forward / input gradient on the first and last 4 images, filter gradient on the full batch)."""
   from compare_gan_b200 import _lib, tape
@@ -69,14 +69,14 @@ its deterministic split-K grouping follows the CTA count), and match the fp32
         lib.set_option(_lib.OPT_TC_EPI, epi)
         xd, wd, bd = dev(K, x, True), dev(K, w, True), dev(K, b, True)
         y = K.conv2d(xd, wd, bd, stride=1, upsample=up)
-        assert lib.get_option(_lib.OPT_LAST_PATH) == 1, "expected the tcgen05 path"
+        assert lib.get_option(_lib.OPT_LAST_PATH) == 1, "expected the tensor-core path"
         gx, gw = tape.backward([(y, dev(K, gy))], [xd, wd], K.add_grad)
         res["pair" if pair else (halo, mt) if epi else "rowwise"] = (y.cpu(), gx.cpu(), gw.cpu())
         del xd, wd, bd, y, gx, gw
-    # the coalescing epilogue (32 x 32 chunks transposed through shared memory) only changes which thread stores a value
+    # the epilogue option (CGAN_OPT_TC_EPI) must not change a value
     for a, c, what in zip(res["rowwise"][:2], res[0, 2][:2], ("forward", "input gradient")):
       np.testing.assert_array_equal(a, c, err_msg="%s: transposing epilogue differs from per-thread rows (%s)" % (name, what))
-    # CTA pairs (cta_group::2, M = 256, each CTA holding half of the weight tile) vs single CTAs: same products, same order
+    # two-CTA clusters sharing the weight tile (CGAN_OPT_TC_PAIR) vs single CTAs: same products, same order
     for a, c, what in zip(res["pair"][:2], res[0, 2][:2], ("forward", "input gradient")):
       assert_close(a, c, 1e-6, "%s: CTA pairs vs single CTAs (%s)" % (name, what))
     for halo in (2, 0):
@@ -341,7 +341,7 @@ def test_tf32_network_parity(case):
     tc_checked = [r for r in checker.results if r[2] == "tcgen05_tf32"]
     assert emulated or len(tc_checked) >= 12, "only %d tensor-core launches in the cycle" % len(tc_checked)
     # identical operands on both sides: what remains is the accumulation — sequential fp32 on the CPU, the tensor core's
-    # fp32 accumulators (measured on B200: up to ~6e-5 rel-L2 at K = 2304, an order above an fp32 FMA chain) — still >10x
+    # fp32 accumulators (up to ~6e-5 rel-L2 at K = 2304, an order above an fp32 FMA chain) — still >10x
     # below what TF32 operand rounding costs, and far below what a wrong tap / offset / epilogue would show (O(1))
     bad = [r for r in checker.results if r[0] > (2e-4 if r[2] == "tcgen05_tf32" else 3e-5) and r[3] > 1e-12]
     assert not bad, "%s: contractions differing from their in-situ CPU recomputation: %s" % (case, sorted(bad, reverse=True)[:5])
