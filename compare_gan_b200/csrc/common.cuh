@@ -17,8 +17,6 @@ struct cgan_ctx {
   int num_sms;
   int tc_mt_max;       // tensor-core kernels: max tiles per CTA sharing one operand tile (CGAN_OPT_TC_MT / env CGAN_TC_MT, default 2)
   int tc_halo;         // 3x3 stride-1 tensor-core convolutions use the halo variant (CGAN_OPT_TC_HALO / env CGAN_TC_HALO, default 1)
-  int tc_pair;         // convolutions run as two-CTA clusters multicasting each weight tile (CGAN_OPT_TC_PAIR / env CGAN_TC_PAIR)
-  int tc_epi;          // accepted and reported only: one epilogue form on sm_90a (CGAN_OPT_TC_EPI / env CGAN_TC_EPI)
   int tc_thin;         // image-side (<= 4 channel) convolutions through 32-wide patch tensors on wgmma (CGAN_OPT_TC_THIN / env CGAN_TC_THIN)
   int last_path;       // CGAN_PATH_* of the most recent contraction (cgan_ctx_get_option(CGAN_OPT_LAST_PATH))
   unsigned* counters;  // CGAN_NUM_COUNTERS zero-initialised tickets for single-launch two-stage reductions (norm.cu)
@@ -99,18 +97,136 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
   return r;
 }
 
-// Optional arguments of the tensor-core convolution launcher cgan_conv_tc (all zero = the plain convolution)
-struct TcExtra {
-  const float* wprep;       // weights already prepared by cgan_tc_prep_weights (shared by several launches)
-  int a_prerounded;         // the activation operand already holds TF32-representable values: skip the in-smem rounding
-  int round_out;            // store TF32-rounded outputs
-  const float* residual;    // + residual (output geometry), before the activation
-  const float* mask;        // (leaky-)ReLU backward fused into the epilogue: out = mask > 0 ? v : mask_leak * v
-  float mask_leak;
-  int nphases;              // > 1: several sub-pixel phases in one launch (tap list = concatenation, see cgan_conv_tc)
+// ---- tap lists of the tensor-core convolutions --------------------------------------------------------------------
+// Tap (kh, kw) of a convolution d multiplies the HWIO weight slice kh * d->kw + kw.  Its signed offset per dimension is
+// t = sign * (k - pad): sign +1 where the forward convolution reads its input relative to the output pixel, -1 for the
+// adjoint (the input gradient reads dy relative to dx).  On a stride-2 grid t splits into t = 2 * half + parity:
+//   TAP_DIRECT  offset t, view 0 (stride 1)
+//   TAP_VIEW    offset half into view 2 * parity_h + parity_w: the operand is read through its four parity phases
+//   TAP_PHASE   offset -half, view = output phase 2 * parity_h + parity_w: output pixel 2i + parity reads pixel i - half
+constexpr int CGAN_TC_MAX_TAPS = 32;
+enum TapRule { TAP_DIRECT, TAP_VIEW, TAP_PHASE };
+
+struct ConvTaps {
+  int ntaps;
+  int off_h[CGAN_TC_MAX_TAPS], off_w[CGAN_TC_MAX_TAPS], wtap[CGAN_TC_MAX_TAPS], view[CGAN_TC_MAX_TAPS];
+  int nphases;              // > 1: the list is grouped by output phase, phase ph owning taps [ph_tap0[ph], ph_tap0[ph + 1])
   int ph_tap0[5];
-  long long ph_base[4];
 };
+
+// false when the kernel has more taps than a list holds
+static inline bool conv_taps(const cgan_conv_desc* d, int sign, TapRule rule, ConvTaps* t) {
+  if (d->kh * d->kw > CGAN_TC_MAX_TAPS) return false;
+  t->ntaps = 0;
+  t->nphases = 1;
+  for (int kh = 0; kh < d->kh; ++kh)
+    for (int kw = 0; kw < d->kw; ++kw) {
+      const int th = sign * (kh - d->pad_t), tw = sign * (kw - d->pad_l), a = th & 1, b = tw & 1;
+      const int i = t->ntaps++;
+      t->wtap[i] = kh * d->kw + kw;
+      if (rule == TAP_DIRECT) {
+        t->off_h[i] = th; t->off_w[i] = tw; t->view[i] = 0;
+      } else {
+        const int s = rule == TAP_VIEW ? 1 : -1;
+        t->off_h[i] = s * (th - a) / 2; t->off_w[i] = s * (tw - b) / 2; t->view[i] = a * 2 + b;
+      }
+    }
+  return true;
+}
+
+// TAP_PHASE taps grouped by output phase (in phase order, each phase in kernel order); false on an empty phase
+static inline bool conv_taps_by_phase(const cgan_conv_desc* d, int sign, ConvTaps* t) {
+  ConvTaps all;
+  if (!conv_taps(d, sign, TAP_PHASE, &all)) return false;
+  t->ntaps = 0;
+  t->nphases = 4;
+  for (int ph = 0; ph < 4; ++ph) {
+    t->ph_tap0[ph] = t->ntaps;
+    for (int i = 0; i < all.ntaps; ++i) {
+      if (all.view[i] != ph) continue;
+      const int j = t->ntaps++;
+      t->off_h[j] = all.off_h[i]; t->off_w[j] = all.off_w[i]; t->wtap[j] = all.wtap[i]; t->view[j] = 0;
+    }
+    if (t->ntaps == t->ph_tap0[ph]) return false;
+  }
+  t->ph_tap0[4] = t->ntaps;
+  return true;
+}
+
+// ---- launch descriptor of the wgmma implicit-GEMM convolution (cgan_conv_tc, conv_tc.cu) ----------------------------
+//   out[base + n*s_n + y*s_h + x*s_w + col] = epilogue(sum_{tap, k} view[tap][n, y + off_h, x + off_w, k] * W[wtap][col][k])
+// for every output pixel (n, y, x), y < gh, x < gw.  Zero-initialise, then fill through the helpers below.
+struct TcConv {
+  // activation operand: `nviews` (1 or 4) views [n, h, w, kdim] of `in`, view v starting at in + view_off[v]
+  const float* in;
+  int nviews;
+  long long view_off[4];
+  long long in_sw, in_sh, in_sn;      // pixel strides (floats)
+  int n, h, w, kdim;
+  int phase_h, phase_w;               // > 0: the four views are the parity phases of a phase_h x phase_w tensor
+  int in_tf32;                        // the operand already holds TF32-representable values: no rounding in shared memory
+  int gh, gw;                         // output pixel grid
+  // weights [taps_total][kdim][ncols] (transpose_w = 1) or [taps_total][ncols][kdim] (transpose_w = 0)
+  const float* wsrc;
+  int taps_total, transpose_w, ncols;
+  int wimg_stride;                    // != 0: batched GEMM, image i multiplies weight slice wtap + i * wimg_stride
+  ConvTaps taps;                      // views index the operand's views; with taps.nphases > 1 phase ph writes at ph_base[ph]
+  // output
+  float* out;
+  long long s_n, s_h, s_w, base;
+  long long ph_base[4];
+  // epilogue: + bias[col] + residual, then ReLU or the (leaky-)ReLU backward gate out = mask > 0 ? v : mask_leak * v,
+  // then TF32 rounding of the stored value
+  const float* bias;
+  const float* residual;
+  const float* mask;
+  float mask_leak;
+  int relu, round_out;
+};
+
+// dense NHWC operand [n, h, w, c]
+static inline void tc_in_dense(TcConv* c, const float* x, int n, int h, int w, int ch) {
+  c->in = x; c->nviews = 1; c->view_off[0] = 0;
+  c->in_sw = ch; c->in_sh = (long long)w * ch; c->in_sn = (long long)h * w * ch;
+  c->n = n; c->h = h; c->w = w; c->kdim = ch;
+}
+// dense NHWC [n, H, W, c] read through its four parity phases: view 2a + b holds the pixels (2i + a, 2j + b)
+static inline void tc_in_phases(TcConv* c, const float* x, int n, int H, int W, int ch) {
+  c->in = x; c->nviews = 4;
+  for (int v = 0; v < 4; ++v) c->view_off[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
+  c->in_sw = 2ll * ch; c->in_sh = 2ll * W * ch; c->in_sn = (long long)H * W * ch;
+  c->n = n; c->h = (H + 1) / 2; c->w = (W + 1) / 2; c->kdim = ch;
+  c->phase_h = H; c->phase_w = W;
+}
+// dense NHWC output over an h x w grid, rows of `ld` floats
+static inline void tc_out_dense(TcConv* c, float* y, int h, int w, int ld) {
+  c->out = y; c->gh = h; c->gw = w;
+  c->s_w = ld; c->s_h = (long long)w * ld; c->s_n = (long long)h * w * ld; c->base = 0;
+}
+// dense NHWC [.., H, W, c] written through its parity phases: an H/2 x W/2 grid, phase 2a + b at pixel (2i + a, 2j + b)
+static inline void tc_out_phases(TcConv* c, float* y, int H, int W, int ch) {
+  c->out = y; c->gh = H / 2; c->gw = W / 2;
+  c->s_w = 2ll * ch; c->s_h = 2ll * W * ch; c->s_n = (long long)H * W * ch; c->base = 0;
+  for (int v = 0; v < 4; ++v) c->ph_base[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
+}
+// the whole epilogue of `ep` (null: none) and whether the activation operand is already TF32-rounded
+static inline void tc_set_epilogue(TcConv* c, const cgan_conv_epilogue* ep, bool in_tf32) {
+  c->in_tf32 = in_tf32 ? 1 : 0;
+  if (!ep) return;
+  c->bias = ep->bias; c->residual = ep->residual; c->mask = ep->mask; c->mask_leak = ep->mask_leak;
+  c->relu = (ep->flags & CGAN_CONV_RELU) ? 1 : 0;
+  c->round_out = (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0;
+}
+
+// Does `ep` still need a cgan_conv_post_epilogue pass after a kernel that applied only the bias (and the ReLU when
+// relu_fused)?
+static inline bool ep_needs_post(const cgan_conv_epilogue* ep, bool relu_fused) {
+  return ep && (ep->residual || ep->mask || (ep->flags & CGAN_CONV_ROUND_OUT) || (!relu_fused && (ep->flags & CGAN_CONV_RELU)));
+}
+
+int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c);
+// geometry the tensor-core convolution accepts for a stride-1 contraction
+bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols);
 
 // internal (C++ linkage) entry points shared between translation units
 int cgan_conv2d_fwd_simt(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const float* bias, float* y,

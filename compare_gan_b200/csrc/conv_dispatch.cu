@@ -2,16 +2,6 @@
 // tensor-core implicit GEMM (conv_tc.cu, math_mode 1) according to the context's math mode and the shape.
 #include "common.cuh"
 
-bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols);
-int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* view_off, long long in_sw, long long in_sh,
-                 long long in_sn, int n, int h, int w, int gh, int gw, int kdim, const float* wsrc, int taps_total,
-                 int transpose_w,
-                 int ncols, int ntaps, const int* off_h, const int* off_w, const int* wtap, const int* amap,
-                 const float* bias, float* out, long long s_n, long long s_h, long long s_w, long long base, int relu,
-                 const int* view_phase_of = nullptr, int wimg_stride = 0, const TcExtra* ex = nullptr);
-int cgan_tc_prep_weights(cgan_ctx* ctx, const float* wsrc, int taps_total, int transpose_w, int ncols, int kdim, float** out);
-int cgan_conv_post_epilogue(cgan_ctx* ctx, float* y, int64_t rows, int c, int ld, const float* residual, const float* mask,
-                            float mask_leak, int relu, int round_out);
 bool cgan_fwd_thin_ok(const cgan_conv_desc* d);
 int cgan_fwd_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y, int relu,
                   int ldy, int round_out);
@@ -41,19 +31,6 @@ int cgan_thin_tc_wgrad_cout(cgan_ctx*, const cgan_conv_desc*, const float* x, co
 
 namespace {
 
-inline TcExtra tc_extra(const cgan_conv_epilogue* ep, bool tf32_in) {
-  TcExtra ex;
-  memset(&ex, 0, sizeof(ex));
-  ex.a_prerounded = tf32_in ? 1 : 0;
-  if (ep) {
-    ex.round_out = (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0;
-    ex.residual = ep->residual; ex.mask = ep->mask; ex.mask_leak = ep->mask_leak;
-  }
-  return ex;
-}
-inline bool ep_has_post(const cgan_conv_epilogue* ep) {
-  return ep && (ep->residual || ep->mask || (ep->flags & (CGAN_CONV_RELU | CGAN_CONV_ROUND_OUT)));
-}
 inline bool al16p(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
@@ -94,7 +71,6 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   const bool ld_ok = ldy == d->cout || ldy % 4 == 0;      // the tensor-core epilogue stores rows of float2 pairs (a multiple of 4 keeps them aligned)
   const bool ptr_ok = al16p(x) && al16p(y) && (!bias || al16p(bias)) && (!ep || ((!ep->residual || al16p(ep->residual)) &&
                                                                                   (!ep->mask || al16p(ep->mask))));
-  TcExtra ex = tc_extra(ep, x_tf32);
   if (ctx->tc_thin && ptr_ok && ld_ok && al16p(w) && !(d->kh == 1 && d->kw == 1)) {
     if (cgan_thin_tc_cin_ok(ctx, d)) {
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
@@ -105,72 +81,46 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
       return cgan_thin_tc_fwd_cout(ctx, d, x, w, ep, y);
     }
   }
+  TcConv c = {};
+  tc_in_dense(&c, x, d->n, d->h, d->w, d->cin);
+  c.wsrc = w; c.taps_total = d->kh * d->kw; c.transpose_w = 1; c.ncols = d->cout;
   // a 1x1 kernel over a zero-inserted input (BigGAN's up-sampling shortcut): phase (0,0) is a plain 1x1 conv written to the
   // even pixels, the other three phases are bias only
   if (ctx->math_mode == 1 && d->stride == 1 && d->upsample && d->kh == 1 && d->kw == 1 && d->oh == 2 * d->h &&
       d->ow == 2 * d->w && d->pad_t == 0 && d->pad_l == 0 && d->cout % 4 == 0 &&
       cgan_tc_shape_ok(d->n, d->h, d->w, d->cin, d->cout) && ptr_ok) {
-    const long long zero = 0;
-    const int o0 = 0, t0 = 0;
-    TcExtra ex0;
-    memset(&ex0, 0, sizeof(ex0));
-    ex0.a_prerounded = ex.a_prerounded;
+    c.taps.ntaps = 1;
+    tc_out_phases(&c, y, d->oh, d->ow, d->cout);
+    tc_set_epilogue(&c, nullptr, x_tf32);
+    c.bias = bias;
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-    int rc = cgan_conv_tc(ctx, x, 1, &zero, d->cin, (long long)d->w * d->cin, (long long)d->h * d->w * d->cin, d->n, d->h,
-                          d->w, d->h, d->w, d->cin, w, 1, 1, d->cout, 1, &o0, &o0, &t0, nullptr, bias, y,
-                          (long long)d->oh * d->ow * d->cout, 2ll * d->ow * d->cout, 2ll * d->cout, 0, 0, nullptr, 0, &ex0);
+    int rc = cgan_conv_tc(ctx, c);
     if (rc) return rc;
     rc = cgan_upsample1x1_bias_phases(ctx, y, bias, d->n, d->oh, d->ow, d->cout);
     if (rc) return rc;
-    if (ep_has_post(ep))
+    if (ep_needs_post(ep, false))
       return cgan_conv_post_epilogue(ctx, y, (int64_t)d->n * d->oh * d->ow, d->cout, d->cout, ep->residual, ep->mask,
-                                     ep->mask_leak, relu, ex.round_out);
+                                     ep->mask_leak, relu, (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0);
     return CGAN_OK;
   }
+  tc_set_epilogue(&c, ep, x_tf32);
   if (ctx->math_mode == 1 && d->stride == 1 && d->kh * d->kw <= 32 && !(d->upsample && (d->kh < 2 || d->kw < 2)) &&
       (!d->upsample || (d->oh == 2 * d->h && d->ow == 2 * d->w)) && d->oh <= (d->upsample ? 2 * d->h : d->h) &&
       d->ow <= (d->upsample ? 2 * d->w : d->w) && cgan_tc_shape_ok(d->n, d->h, d->w, d->cin, d->cout) && ptr_ok &&
       !(d->upsample && d->cout % 4 != 0) && ld_ok) {
-    int oh[32], ow[32], wt[32];
-    const long long zero = 0;
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
     if (!d->upsample) {
-      int nt = 0;
-      for (int kh = 0; kh < d->kh; ++kh)
-        for (int kw = 0; kw < d->kw; ++kw) {
-          oh[nt] = kh - d->pad_t; ow[nt] = kw - d->pad_l; wt[nt] = kh * d->kw + kw; ++nt;
-        }
-      return cgan_conv_tc(ctx, x, 1, &zero, d->cin, (long long)d->w * d->cin, (long long)d->h * d->w * d->cin, d->n, d->h,
-                          d->w, d->oh, d->ow, d->cin, w, d->kh * d->kw, 1, d->cout, nt, oh, ow, wt, nullptr, bias, y,
-                          (long long)d->oh * d->ow * ldy, (long long)d->ow * ldy, ldy, 0, relu, nullptr, 0, &ex);
+      conv_taps(d, 1, TAP_DIRECT, &c.taps);
+      tc_out_dense(&c, y, d->oh, d->ow, ldy);
+      return cgan_conv_tc(ctx, c);
     }
-    // conv over the zero-inserted 2x upsampled input (resnet_ops.py:35-56, 122-130) as four sub-pixel phases: output
-    // pixel (2i+a, 2j+b) only sees the taps whose virtual input coordinate 2i+a+kh-pad is even -> real pixel i+dh.
-    // The weights are prepared once for the four launches.
-    // One launch (grid.z = phase), one weight preparation.
-    int nt = 0;
-    ex.nphases = 4;
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) {
-        const int ph = a * 2 + b;
-        ex.ph_tap0[ph] = nt;
-        ex.ph_base[ph] = ((long long)a * d->ow + b) * d->cout;
-        for (int kh = 0; kh < d->kh; ++kh) {
-          int vh = a + kh - d->pad_t;
-          if (vh & 1) continue;
-          for (int kw = 0; kw < d->kw; ++kw) {
-            int vw = b + kw - d->pad_l;
-            if (vw & 1) continue;
-            oh[nt] = vh / 2; ow[nt] = vw / 2;      // exact: vh, vw even (possibly negative)
-            wt[nt] = kh * d->kw + kw; ++nt;
-          }
-        }
-        if (nt == ex.ph_tap0[ph]) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: empty sub-pixel phase%s", "cgan_conv2d_fwd");
-      }
-    ex.ph_tap0[4] = nt;
-    return cgan_conv_tc(ctx, x, 1, &zero, d->cin, (long long)d->w * d->cin, (long long)d->h * d->w * d->cin, d->n,
-                        d->h, d->w, d->h, d->w, d->cin, w, d->kh * d->kw, 1, d->cout, nt, oh, ow, wt, nullptr, bias, y,
-                        (long long)d->oh * d->ow * d->cout, 2ll * d->ow * d->cout, 2ll * d->cout, 0, relu, nullptr, 0, &ex);
+    // conv over the zero-inserted 2x upsampled input (resnet_ops.py:35-56, 122-130) as four sub-pixel phases in one
+    // launch (grid.z = phase): output pixel (2i+a, 2j+b) only sees the taps whose virtual input coordinate 2i+a+kh-pad is
+    // even -> real pixel i+dh.
+    if (!conv_taps_by_phase(d, -1, &c.taps))
+      return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: empty sub-pixel phase%s", "cgan_conv2d_fwd");
+    tc_out_phases(&c, y, d->oh, d->ow, d->cout);
+    return cgan_conv_tc(ctx, c);
   }
   // stride 2 (SNDCGAN D, sndcgan.py:109-121): the input is read through its four (row, column) parity phases, each a
   // strided TMA view of the output's spatial size; tap (kh,kw) lands in phase ((kh-pad_t)&1, (kw-pad_l)&1).
@@ -178,25 +128,14 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   if (ctx->math_mode == 1 && d->stride == 2 && !d->upsample && d->kh * d->kw <= 32 && d->h >= 2 && d->w >= 2 &&
       (d->oh - 1) * 2 + d->kh - d->pad_t <= d->h + d->kh && cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cin, d->cout) &&
       ptr_ok && ld_ok) {
-    int oh[32], ow[32], wt[32], am[32], nt = 0;
-    const int hw[2] = {d->h, d->w};
-    long long voff[4];
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) voff[a * 2 + b] = ((long long)a * d->w + b) * d->cin;
-    for (int kh = 0; kh < d->kh; ++kh) {
-      int th = kh - d->pad_t, a = th & 1;
-      for (int kw = 0; kw < d->kw; ++kw) {
-        int tw = kw - d->pad_l, b = tw & 1;
-        oh[nt] = (th - a) / 2; ow[nt] = (tw - b) / 2; wt[nt] = kh * d->kw + kw; am[nt] = a * 2 + b; ++nt;
-      }
-    }
+    tc_in_phases(&c, x, d->n, d->h, d->w, d->cin);
+    conv_taps(d, 1, TAP_VIEW, &c.taps);
+    tc_out_dense(&c, y, d->oh, d->ow, ldy);
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-    return cgan_conv_tc(ctx, x, 4, voff, 2ll * d->cin, 2ll * d->w * d->cin, (long long)d->h * d->w * d->cin, d->n,
-                        (d->h + 1) / 2, (d->w + 1) / 2, d->oh, d->ow, d->cin, w, d->kh * d->kw, 1, d->cout, nt, oh, ow, wt, am,
-                        bias, y, (long long)d->oh * d->ow * ldy, (long long)d->ow * ldy, ldy, 0, relu, hw, 0, &ex);
+    return cgan_conv_tc(ctx, c);
   }
   // exact-fp32 paths: residual / mask / rounding are applied by one extra pointwise pass
-  bool post = ep && (ep->residual || ep->mask || (ep->flags & CGAN_CONV_ROUND_OUT));
+  bool post = ep_needs_post(ep, true);
   int rc;
   if (cgan_pw_thin_ok(d) && ptr_ok && al16p(w) && ldy % 4 == 0 && !(ep && ep->mask)) {
     // pointwise conv over <= 4 channels: one streaming kernel with residual add, ReLU and rounding fused
@@ -232,7 +171,6 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
   const bool dy_tf32 = ep && (ep->flags & CGAN_CONV_IN_TF32);
   const bool ptr_ok = al16p(dy) && al16p(dx) && (!bias || al16p(bias)) &&
                       (!ep || ((!ep->residual || al16p(ep->residual)) && (!ep->mask || al16p(ep->mask))));
-  TcExtra ex = tc_extra(ep, dy_tf32);
   const bool geom = d->oh == (d->upsample ? 2 * d->h : d->h) && d->ow == (d->upsample ? 2 * d->w : d->w);
   if (ctx->tc_thin && ptr_ok && al16p(w) && !(d->kh == 1 && d->kw == 1)) {
     if (cgan_thin_tc_cout_ok(ctx, d)) {          // dy has <= 4 channels (the generator's image conv)
@@ -244,79 +182,48 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
       return cgan_thin_tc_dgrad_cin(ctx, d, dy, w, ep, dx);
     }
   }
+  // dx[n,ih,iw,ci] = sum_{kh,kw,co} dy[n, oh, ow, co] * w[kh,kw,ci,co]: HWIO is already [tap][row=ci][k=co], i.e.
+  // K-major for this contraction (no transpose).
+  TcConv c = {};
+  tc_in_dense(&c, dy, d->n, d->oh, d->ow, d->cout);
+  c.wsrc = w; c.taps_total = d->kh * d->kw; c.transpose_w = 0; c.ncols = d->cin;
+  tc_set_epilogue(&c, ep, dy_tf32);
   if (ctx->math_mode == 1 && d->stride == 1 && d->kh * d->kw <= 32 && geom &&
       cgan_tc_shape_ok(d->n, d->h, d->w, d->cout, d->cin) && ptr_ok) {
-    // dx[n,ih,iw,ci] = sum_{kh,kw,co} dy[n, oh, ow, co] * w[kh,kw,ci,co]: HWIO is already [tap][row=ci][k=co], i.e.
-    // K-major for this contraction (no transpose).
-    int oh[32], ow[32], wt[32], am[32], nt = 0;
-    long long voff[4] = {0, 0, 0, 0};
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
+    tc_out_dense(&c, dx, d->h, d->w, d->cin);
     if (!d->upsample) {
-      // oh = ih + pad_t - kh
-      for (int kh = 0; kh < d->kh; ++kh)
-        for (int kw = 0; kw < d->kw; ++kw) {
-          oh[nt] = d->pad_t - kh; ow[nt] = d->pad_l - kw; wt[nt] = kh * d->kw + kw; am[nt] = 0; ++nt;
-        }
-      return cgan_conv_tc(ctx, dy, 1, voff, d->cout, (long long)d->ow * d->cout, (long long)d->oh * d->ow * d->cout, d->n,
-                          d->h, d->w, d->h, d->w, d->cout, w, d->kh * d->kw, 0, d->cin, nt, oh, ow, wt, am, bias, dx,
-                          (long long)d->h * d->w * d->cin, (long long)d->w * d->cin, d->cin, 0, relu, nullptr, 0, &ex);
+      conv_taps(d, -1, TAP_DIRECT, &c.taps);          // oh = ih + pad_t - kh
+      return cgan_conv_tc(ctx, c);
     }
     // zero-inserted input: the real pixel ih sits at virtual row 2*ih; tap kh reaches output row oh = 2*ih + pad_t - kh,
     // i.e. sub-pixel phase a = (pad_t - kh) & 1 of dy at phase-row ih + (pad_t - kh - a)/2.  The four phases are four
     // strided TMA views of dy.
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) voff[a * 2 + b] = ((long long)a * d->ow + b) * d->cout;
-    for (int kh = 0; kh < d->kh; ++kh) {
-      int th = d->pad_t - kh, a = th & 1;
-      for (int kw = 0; kw < d->kw; ++kw) {
-        int tw = d->pad_l - kw, b = tw & 1;
-        oh[nt] = (th - a) / 2; ow[nt] = (tw - b) / 2; wt[nt] = kh * d->kw + kw; am[nt] = a * 2 + b; ++nt;
-      }
-    }
-    return cgan_conv_tc(ctx, dy, 4, voff, 2ll * d->cout, 2ll * d->ow * d->cout, (long long)d->oh * d->ow * d->cout, d->n,
-                        d->h, d->w, d->h, d->w, d->cout, w, d->kh * d->kw, 0, d->cin, nt, oh, ow, wt, am, bias, dx,
-                        (long long)d->h * d->w * d->cin, (long long)d->w * d->cin, d->cin, 0, relu, nullptr, 0, &ex);
+    tc_in_phases(&c, dy, d->n, d->oh, d->ow, d->cout);
+    conv_taps(d, -1, TAP_VIEW, &c.taps);
+    return cgan_conv_tc(ctx, c);
   }
   // stride 2 (also tf.nn.conv2d_transpose of SNDCGAN's generator, arch_ops.py:588-589): input pixel 2i+a only receives
-  // the taps with kh = a + pad_t (mod 2), from output row i + (a + pad_t - kh)/2 -> four launches, one per input phase,
-  // each writing a strided quarter of dx; the weights are prepared once.
+  // the taps with kh = a + pad_t (mod 2), from output row i + (a + pad_t - kh)/2 -> four input phases in one launch
+  // (grid.z = phase), each writing a strided quarter of dx.
   if (ctx->math_mode == 1 && d->stride == 2 && !d->upsample && d->kh * d->kw <= 16 && !(d->h & 1) && !(d->w & 1) &&
       d->oh == d->h / 2 && d->ow == d->w / 2 && d->kh >= 2 && d->kw >= 2 &&
       cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cout, d->cin) && ptr_ok && d->cin % 4 == 0) {
-    const long long zero = 0;
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-    int oh[32], ow[32], wt[32], nt = 0;
-    ex.nphases = 4;
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) {
-        const int ph = a * 2 + b;
-        ex.ph_tap0[ph] = nt;
-        ex.ph_base[ph] = ((long long)a * d->w + b) * d->cin;
-        for (int kh = 0; kh < d->kh; ++kh) {
-          int th = a + d->pad_t - kh;
-          if (th & 1) continue;
-          for (int kw = 0; kw < d->kw; ++kw) {
-            int tw = b + d->pad_l - kw;
-            if (tw & 1) continue;
-            oh[nt] = th / 2; ow[nt] = tw / 2; wt[nt] = kh * d->kw + kw; ++nt;
-          }
-        }
-        if (nt == ex.ph_tap0[ph]) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: empty phase%s", "cgan_conv2d_dgrad");
-      }
-    ex.ph_tap0[4] = nt;
-    return cgan_conv_tc(ctx, dy, 1, &zero, d->cout, (long long)d->ow * d->cout, (long long)d->oh * d->ow * d->cout,
-                        d->n, d->oh, d->ow, d->oh, d->ow, d->cout, w, d->kh * d->kw, 0, d->cin, nt, oh, ow, wt, nullptr,
-                        bias, dx, (long long)d->h * d->w * d->cin, 2ll * d->w * d->cin, 2ll * d->cin, 0, relu, nullptr, 0, &ex);
+    if (!conv_taps_by_phase(d, 1, &c.taps))
+      return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: empty phase%s", "cgan_conv2d_dgrad");
+    tc_out_phases(&c, dx, d->h, d->w, d->cin);
+    return cgan_conv_tc(ctx, c);
   }
   ctx->last_path = CGAN_PATH_SIMT_FP32;
   int rc = cgan_conv2d_dgrad_simt(ctx, d, dy, w, dx);
   if (rc) return rc;
-  if (bias || ep_has_post(ep)) {
+  if (bias || ep_needs_post(ep, false)) {
     if (bias) {
       rc = cgan_bias_add(ctx, dx, dx, bias, (int64_t)d->n * d->h * d->w, d->cin);
       if (rc) return rc;
     }
-    if (ep_has_post(ep))
+    if (ep_needs_post(ep, false))
       return cgan_conv_post_epilogue(ctx, dx, (int64_t)d->n * d->h * d->w, d->cin, d->cin, ep->residual, ep->mask,
                                      ep->mask_leak, relu, (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0);
   }
@@ -374,11 +281,13 @@ int cgan_gemm_batched(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float 
     const bool nt = tb && ldb == k && sb == (int64_t)n * k;        // B[i] stored [n, k]  (K-major already)
     const bool nn = !tb && ldb == n && sb == (int64_t)k * n;       // B[i] stored [k, n]  (transposed by the prep kernel)
     if (nt || nn) {
-      const long long zero = 0;
-      const int o0 = 0;
+      TcConv g = {};
+      tc_in_dense(&g, a, batch, h, w, k);
+      g.wsrc = b; g.taps_total = batch; g.transpose_w = nn ? 1 : 0; g.ncols = n; g.wimg_stride = 1;
+      g.taps.ntaps = 1;                // one tap at offset 0: image i multiplies weight slice i
+      tc_out_dense(&g, c, h, w, n);
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-      return cgan_conv_tc(ctx, a, 1, &zero, k, (long long)w * k, (long long)m * k, batch, h, w, h, w, k, b, batch, nn ? 1 : 0, n,
-                          1, &o0, &o0, &o0, nullptr, nullptr, c, (long long)m * n, (long long)w * n, n, 0, 0, nullptr, 1);
+      return cgan_conv_tc(ctx, g);
     }
   }
   if (ctx->math_mode == 1 && plain && ta && !tb && rows_as_grid(k, &h, &w) && lda == m && sa == (int64_t)k * m && ldb == n &&

@@ -84,7 +84,7 @@ __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int t, int& ow
   ow0 = tw * p.bw; oh0 = th * p.bh; n0 = tn * p.bni;
 }
 
-__device__ __forceinline__ float tc_epilogue_one(const TcParams& p, float v, int col, long long off) {
+__device__ __forceinline__ float epilogue_one(const TcParams& p, float v, int col, long long off) {
   if (p.bias) v += p.bias[col];
   if (p.residual) v += p.residual[off];
   if (p.relu) v = fmaxf(v, 0.f);
@@ -97,7 +97,7 @@ __device__ __forceinline__ float tc_epilogue_one(const TcParams& p, float v, int
 // 8j + 2 (lane % 4) + {0, 1}.  A quad of lanes writes 32 contiguous bytes of one output row.  Rows beyond the box (stale
 // smem) and pixels outside the grid are computed but never stored.
 template <int BN>
-__device__ __forceinline__ void tc_epilogue(const TcParams& p, const float* acc, int tile, int nb0, int wg, int warp, int lane,
+__device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* acc, int tile, int nb0, int wg, int warp, int lane,
                                             long long out_base) {
   int ow0, oh0, n0;
   tc_tile_origin(p, tile, ow0, oh0, n0);
@@ -128,8 +128,8 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, const float* acc,
         if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
         *reinterpret_cast<float2*>(p.out + off) = v;
       } else {        // odd column count or odd row offsets (e.g. the 256->3 image conv): element by element
-        p.out[off] = tc_epilogue_one(p, v.x, nb0 + c, off);
-        if (nb0 + c + 1 < p.cout) p.out[off + 1] = tc_epilogue_one(p, v.y, nb0 + c + 1, off + 1);
+        p.out[off] = epilogue_one(p, v.x, nb0 + c, off);
+        if (nb0 + c + 1 < p.cout) p.out[off + 1] = epilogue_one(p, v.y, nb0 + c + 1, off + 1);
       }
     }
   }
@@ -145,12 +145,7 @@ __device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, i
   }
 }
 
-// CL = 2: the CTA runs in a cluster of two neighbouring pixel-tile groups that share the weight tile: each CTA loads half
-// of its rows and multicasts them to both, so a k-block costs each SM MT*16 KB + BN*64 B of L2 -> SM traffic instead of
-// MT*16 KB + BN*128 B (the kernel is bound by that feed at BN = 256).  A stage is refilled only when the consumers of BOTH
-// CTAs have released it (empty barrier count 2 x 2); the CTAs meet at cluster barriers after initialising the barriers and
-// before exiting, so no multicast or remote arrive ever targets a CTA that is not running.
-template <int BN, int MT, int CL>
+template <int BN, int MT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -165,10 +160,9 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tap0 = p.ph_tap0[blockIdx.z];
   const int num_kb = (p.ph_tap0[blockIdx.z + 1] - tap0) * p.kchunks;
-  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
 
   // this CTA's pixel tiles: [tile0, tile0 + nt_here).  They all multiply the same weight tile, which is therefore
-  // fetched from L2 once per k-block for MT*128 pixels.  (A cluster's second CTA may lie past the last tile: nt_here = 0.)
+  // fetched from L2 once per k-block for MT*128 pixels.
   const int tile0 = blockIdx.x * MT;
   const int nt_here = max(0, min(MT, p.tiles_total - tile0));
   const int nb0 = blockIdx.y * BN;          // first output channel of this CTA
@@ -176,11 +170,11 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2 * CL);            // one arrive per consumer warpgroup of every CTA that fills the stage
+      mbar_init(&empty_bar[s], 2);            // one arrive per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (CL == 2) cluster_sync_all(); else __syncthreads();
+  __syncthreads();
 
   if (warp == TC_CWARPS) {
     // ===== TMA producer =====
@@ -201,13 +195,8 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
           tma_load_4d(sa + i * TC_A_BYTES, &tm_as.m[p.amap[tap]], &full_bar[stage], kc * TC_BK, ow0 + p.off_w[tap],
                       oh0 + p.off_h[tap], n0);
         }
-        if (CL == 2) {          // this CTA's half of the weight rows, into both CTAs (no batched GEMM here)
-          tma_load_3d_multicast(sb + rank * (BN / 2) * 128, &tm_b, &full_bar[stage], kc * TC_BK, nb0 + (int)rank * (BN / 2),
-                                p.wtap[tap], (uint16_t)3);
-        } else {
-          tc_tile_origin(p, tile0, ow0, oh0, n0);   // batched GEMM: all tiles of a CTA lie in one image (host guarantees)
-          tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
-        }
+        tc_tile_origin(p, tile0, ow0, oh0, n0);   // batched GEMM: all tiles of a CTA lie in one image (host guarantees)
+        tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
     }
@@ -250,10 +239,7 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
       for (int t = 0; t < MT; ++t)
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
-      if (prev >= 0 && q == 0) {
-        mbar_arrive(&empty_bar[prev]);
-        if (CL == 2) mbar_arrive_cluster(&empty_bar[prev], rank ^ 1);
-      }
+      if (prev >= 0 && q == 0) mbar_arrive(&empty_bar[prev]);
       prev = stage;
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
@@ -262,10 +248,9 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
     for (int t = 0; t < MT; ++t) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
-      if (t < nt_here) tc_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z]);
+      if (t < nt_here) tile_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z]);
     }
   }
-  if (CL == 2) cluster_sync_all();
 }
 
 // ---- halo variant ------------------------------------------------------------------------------------------------
@@ -393,7 +378,7 @@ conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
   for (int t = 0; t < MT; ++t) {
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
-    if (t < nt_here) tc_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.base);
+    if (t < nt_here) tile_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.base);
   }
 }
 
@@ -457,52 +442,57 @@ inline int tc_vec2(const TcParams& p) {
   return (odd & 1) ? 0 : 1;
 }
 
-// kind: 0 plain kernel, 1 plain kernel in two-CTA clusters (grid.x even; `b` maps half of the weight tile), 2 halo kernel
+// Weights -> TF32-rounded (nearest) K-major [taps_total][ncols_pad][kdim_pad] in the context workspace
+int prep_weights(cgan_ctx* ctx, const TcConv& c, int kdim_pad, int ncols_pad, float** out) {
+  void* ws = nullptr;
+  int rc = cgan_ws(ctx, (size_t)c.taps_total * ncols_pad * kdim_pad * sizeof(float), &ws);
+  if (rc) return rc;
+  float* wt = reinterpret_cast<float*>(ws);
+  long long tot = (long long)c.taps_total * ncols_pad * kdim_pad;
+  long long blocks = (tot + 255) / 256, cap = (long long)ctx->num_sms * 8;
+  wprep_kernel<<<(int)(blocks > cap ? cap : blocks), 256, 0, ctx->stream>>>(wt, c.wsrc, c.taps_total, c.ncols, ncols_pad, c.kdim,
+                                                                             kdim_pad, c.transpose_w);
+  CGAN_LAUNCHED(ctx);
+  *out = wt;
+  return CGAN_OK;
+}
+
+// 3-D map {k, column, tap} of the prepared weights, 128B-swizzled boxes of 32 channels x bn columns of one tap
+bool make_weight_map(CUtensorMap* tm, float* wt, int kdim_pad, int ncols_pad, int taps_total, int bn) {
+  cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
+  cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
+  cuuint32_t box[3] = {TC_BK, (cuuint32_t)bn, 1};
+  cuuint32_t es[3] = {1, 1, 1};
+  return get_encode()(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// halo: the halo kernel, reading the activation box through as.m[0]
 template <int BN, int MT>
-int tc_launch_t(cgan_ctx* ctx, int kind, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& a1,
-                const CUtensorMap& b, const TcParams& p) {
-  static bool attr_set[3] = {false, false, false};
-  if (kind == 2) {
-    if (!attr_set[2]) {
-      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_halo_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set[2] = true;
-    }
-    conv_tc_halo_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(a1, b, p);
-  } else if (kind == 1) {
+int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
+  static bool attr_set[2] = {false, false};
+  if (halo) {
     if (!attr_set[1]) {
-      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_halo_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set[1] = true;
     }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    CGAN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MT, 2>, as, b, p));
+    conv_tc_halo_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as.m[0], b, p);
   } else {
     if (!attr_set[0]) {
-      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set[0] = true;
     }
-    conv_tc_kernel<BN, MT, 1><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p);
+    conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p);
   }
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }
 
 // the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS
-int tc_launch(cgan_ctx* ctx, int kind, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& a1, const CUtensorMap& b,
-              const TcParams& p) {
+int tc_launch(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
 #define TC_CASE(BN, MT) \
-  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, kind, grid, smem, as, a1, b, p);
+  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p);
   TC_CASE(32, 1) TC_CASE(64, 1) TC_CASE(96, 1) TC_CASE(128, 1) TC_CASE(160, 1) TC_CASE(192, 1) TC_CASE(224, 1)
   TC_CASE(256, 1) TC_CASE(32, 2) TC_CASE(64, 2) TC_CASE(96, 2) TC_CASE(128, 2)
 #undef TC_CASE
@@ -511,7 +501,6 @@ int tc_launch(cgan_ctx* ctx, int kind, dim3 grid, size_t smem, const AMaps& as, 
 
 }  // namespace
 
-// Geometry the tensor-core path accepts for a stride-1 convolution-like contraction.
 bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols) {
   if (n < 1 || h < 1 || w < 1 || ncols < 1) return false;
   if (kdim < 8 || kdim % 4 != 0) return false;           // TMA needs 16-byte pixel strides; K is zero-padded to 32
@@ -520,52 +509,18 @@ bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols) {
   return bn != 0 && bn % 32 == 0;
 }
 
-// Weights -> TF32-rounded (nearest) K-major [taps_total][ncols_pad][kdim_pad] in the context workspace.  Split from the
-// launch so that a convolution over a zero-inserted input prepares its weights ONCE for its four sub-pixel phases.
-int cgan_tc_prep_weights(cgan_ctx* ctx, const float* wsrc, int taps_total, int transpose_w, int ncols, int kdim, float** out) {
-  const int kdim_pad = (kdim + TC_BK - 1) / TC_BK * TC_BK;
-  const int ncols_pad = (ncols + 31) / 32 * 32;
-  void* ws = nullptr;
-  size_t wbytes = (size_t)taps_total * ncols_pad * kdim_pad * sizeof(float);
-  int rc = cgan_ws(ctx, wbytes, &ws);
-  if (rc) return rc;
-  float* wt = reinterpret_cast<float*>(ws);
-  long long tot = (long long)taps_total * ncols_pad * kdim_pad;
-  long long blocks = (tot + 255) / 256, cap = (long long)ctx->num_sms * 8;
-  wprep_kernel<<<(int)(blocks > cap ? cap : blocks), 256, 0, ctx->stream>>>(wt, wsrc, taps_total, ncols, ncols_pad, kdim,
-                                                                             kdim_pad, transpose_w);
-  CGAN_LAUNCHED(ctx);
-  *out = wt;
-  return CGAN_OK;
-}
-
-// in: fp32 NHWC activations seen through `nviews` views of logical size [n, h, w, kdim] (view v starts at
-// in + view_off[v], pixel strides sw/sh/sn floats) — one view for ordinary convs, the four sub-pixel phases of a
-// 2x-upsampled gradient for the input gradient of a conv over a zero-inserted input.
-// wsrc: weights [taps_total][kdim][ncols] (transpose_w=1) or [taps_total][ncols][kdim] (transpose_w=0); ignored when
-// ex->wprep holds the output of cgan_tc_prep_weights for the same weights.
-// taps: `ntaps` entries (off_h, off_w, weight slice, view).  Output pixel (n, y, x), y < gh, x < gw, is written at
-// out + base + n*s_n + y*s_h + x*s_w (+ channel).
-int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* view_off, long long in_sw, long long in_sh,
-                 long long in_sn, int n, int h, int w, int gh, int gw, int kdim, const float* wsrc, int taps_total,
-                 int transpose_w,
-                 int ncols, int ntaps, const int* off_h, const int* off_w, const int* wtap, const int* amap,
-                 const float* bias, float* out, long long s_n, long long s_h, long long s_w, long long base, int relu,
-                 const int* view_phase_of, int wimg_stride, const TcExtra* ex) {
-  // ex->nphases > 1: the `ntaps` taps are the concatenation of the tap lists of nphases sub-pixel phases
-  // (ex->ph_tap0[0..nphases]), phase ph writing at element offset ex->ph_base[ph] instead of `base`; one launch, grid.z
-  // wimg_stride != 0: batched GEMM — image i multiplies weight slice wtap + i*wimg_stride (needs one image per tile)
-  // view_phase_of: {H, W} of the tensor whose four stride-2 parity phases the views are (nullptr: all views h x w)
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled unavailable%s", "cgan_conv_tc");
-  if (ntaps > TC_MAX_TAPS || nviews > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: too many taps/views%s", "cgan_conv_tc");
+int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
+  if (!get_encode()) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled unavailable%s", "cgan_conv_tc");
+  const ConvTaps& tp = c.taps;
+  if (tp.ntaps > TC_MAX_TAPS || c.nviews > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: too many taps/views%s", "cgan_conv_tc");
+  const int n = c.n, h = c.h, w = c.w, kdim = c.kdim, gh = c.gh, gw = c.gw, ntaps = tp.ntaps;
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.ntaps = ntaps;
   const int kdim_pad = (kdim + TC_BK - 1) / TC_BK * TC_BK;
   p.kchunks = kdim_pad / TC_BK;
   for (int i = 0; i < ntaps; ++i) {
-    p.off_h[i] = off_h[i]; p.off_w[i] = off_w[i]; p.wtap[i] = wtap[i]; p.amap[i] = amap ? amap[i] : 0;
+    p.off_h[i] = tp.off_h[i]; p.off_w[i] = tp.off_w[i]; p.wtap[i] = tp.wtap[i]; p.amap[i] = tp.view[i];
   }
   int tiles_n;
   // the pixel grid that is tiled (gh x gw: the OUTPUT extent) may differ from the extent of the input views (h x w):
@@ -573,42 +528,38 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   tc_geometry(n, gh, gw, &p.bw, &p.bh, &p.bni, &p.tiles_w, &p.tiles_h, &tiles_n);
   p.rows_used = p.bw * p.bh * p.bni;
   p.img_n = n; p.img_h = gh; p.img_w = gw;
-  p.relu = relu;
-  p.round_a = (ex && ex->a_prerounded) ? 0 : 1;
-  if (ex) {
-    p.round_out = ex->round_out; p.residual = ex->residual; p.mask = ex->mask; p.mask_leak = ex->mask_leak;
-  }
+  p.relu = c.relu;
+  p.round_a = c.in_tf32 ? 0 : 1;
+  p.round_out = c.round_out; p.residual = c.residual; p.mask = c.mask; p.mask_leak = c.mask_leak;
   p.nphases = 1;
   p.ph_tap0[0] = 0; p.ph_tap0[1] = ntaps;
-  p.ph_base[0] = base;
-  if (ex && ex->nphases > 1) {
-    if (ex->nphases > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: more than four phases%s", "cgan_conv_tc");
-    p.nphases = ex->nphases;
-    for (int i = 0; i <= ex->nphases; ++i) p.ph_tap0[i] = ex->ph_tap0[i];
-    for (int i = 0; i < ex->nphases; ++i) p.ph_base[i] = ex->ph_base[i];
+  p.ph_base[0] = c.base;
+  if (tp.nphases > 1) {
+    if (tp.nphases > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: more than four phases%s", "cgan_conv_tc");
+    p.nphases = tp.nphases;
+    for (int i = 0; i <= tp.nphases; ++i) p.ph_tap0[i] = tp.ph_tap0[i];
+    for (int i = 0; i < tp.nphases; ++i) p.ph_base[i] = c.ph_base[i];
   }
-  p.wimg_stride = wimg_stride;
-  if (wimg_stride != 0 && p.bni != 1)
+  p.wimg_stride = c.wimg_stride;
+  if (c.wimg_stride != 0 && p.bni != 1)
     return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: batched GEMM needs >= 128 rows per matrix%s", "cgan_conv_tc");
-  const int ncols_pad = (ncols + 31) / 32 * 32;
+  const int ncols_pad = (c.ncols + 31) / 32 * 32;
   p.bn = tc_pick_bn_occupancy(ncols_pad, (long long)p.tiles_w * p.tiles_h * tiles_n, ctx->num_sms);
-  p.cout = ncols;
-  p.s_n = s_n; p.s_h = s_h; p.s_w = s_w; p.base = base;
-  p.out = out;
-  p.bias = bias;
+  p.cout = c.ncols;
+  p.s_n = c.s_n; p.s_h = c.s_h; p.s_w = c.s_w; p.base = c.base;
+  p.out = c.out;
+  p.bias = c.bias;
 
-  float* wt = (ex && ex->wprep) ? const_cast<float*>(ex->wprep) : nullptr;
-  if (!wt) {
-    int rc = cgan_tc_prep_weights(ctx, wsrc, taps_total, transpose_w, ncols, kdim, &wt);
-    if (rc) return rc;
-  }
+  float* wt = nullptr;
+  int rc = prep_weights(ctx, c, kdim_pad, ncols_pad, &wt);
+  if (rc) return rc;
 
   // ---- halo variant: three taps of a kernel column share one (bh+2)-row activation box --------------------------------
   // Used where the activation operand still has to be rounded in shared memory (the halo box cuts that work 9 -> 3 x
   // (bh+2)/bh per chunk); a pre-rounded operand streams through the per-tap kernel.  CGAN_OPT_TC_HALO = 2 forces it
   // everywhere (tests).
   const bool halo_wanted = ctx->tc_halo == 2 || (ctx->tc_halo == 1 && p.round_a && ncols_pad >= 256);
-  if (halo_wanted && p.nphases == 1 && nviews == 1 && wimg_stride == 0 && ntaps == 9 && gh == h && gw == w && !view_phase_of) {
+  if (halo_wanted && p.nphases == 1 && c.nviews == 1 && c.wimg_stride == 0 && ntaps == 9 && gh == h && gw == w) {
     int hbw = 0, hbh = 0;
     if (w % 32 == 0) { hbw = 32; hbh = 4; } else if (w == 16) { hbw = 16; hbh = 8; }
     // group the taps by horizontal offset; each group must be three vertically consecutive taps
@@ -617,13 +568,13 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
     for (int i = 0; ok && i < ntaps; ++i) {
       int g = -1;
       for (int j = 0; j < ng; ++j)
-        if (gw_off[j] == off_w[i]) g = j;
+        if (gw_off[j] == tp.off_w[i]) g = j;
       if (g < 0) {
         if (ng == 3) { ok = false; break; }
-        g = ng++; gw_off[g] = off_w[i]; gh0[g] = off_h[i];
+        g = ng++; gw_off[g] = tp.off_w[i]; gh0[g] = tp.off_h[i];
       }
       if (gcnt[g] == 3) { ok = false; break; }
-      if (off_h[i] < gh0[g]) gh0[g] = off_h[i];
+      if (tp.off_h[i] < gh0[g]) gh0[g] = tp.off_h[i];
       gtap[g][gcnt[g]++] = i;
     }
     ok = ok && ng == 3;
@@ -631,9 +582,9 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
       if (gcnt[g] != 3) { ok = false; break; }
       int ordered[3] = {-1, -1, -1};
       for (int j = 0; j < 3; ++j) {
-        int dh = off_h[gtap[g][j]] - gh0[g];
+        int dh = tp.off_h[gtap[g][j]] - gh0[g];
         if (dh < 0 || dh > 2 || ordered[dh] >= 0) { ok = false; break; }
-        ordered[dh] = wtap[gtap[g][j]];
+        ordered[dh] = tp.wtap[gtap[g][j]];
       }
       for (int j = 0; ok && j < 3; ++j) p.h_wtap[g][j] = ordered[j];
       p.h_off_w[g] = gw_off[g]; p.h_off_h0[g] = gh0[g];
@@ -667,22 +618,17 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
       ok = p.sb_stages >= 2;
       if (ok) {
         p.tiles_total = (int)tiles_total;
-        CUtensorMap tm_a, tm_bh;
-        if (!make_act_map(&tm_a, in + view_off[0], kdim, w, h, n, in_sw, in_sh, in_sn, hbw, hbh + 2, 1))
+        AMaps tm_a;
+        CUtensorMap tm_b;
+        memset(&tm_a, 0, sizeof(tm_a));
+        if (!make_act_map(&tm_a.m[0], c.in + c.view_off[0], kdim, w, h, n, c.in_sw, c.in_sh, c.in_sn, hbw, hbh + 2, 1))
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A halo) failed%s", "cgan_conv_tc");
-        cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
-        cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
-        cuuint32_t box[3] = {TC_BK, (cuuint32_t)p.bn, 1};
-        cuuint32_t es[3] = {1, 1, 1};
-        if (enc(&tm_bh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        if (!make_weight_map(&tm_b, wt, kdim_pad, ncols_pad, c.taps_total, p.bn))
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
         p.vec2 = tc_vec2(p);
         size_t smem = (size_t)p.sa_stages * p.mt * p.a_halo_bytes + (size_t)p.sb_stages * b_bytes + 1024 + 512;
         dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles);
-        AMaps unused;
-        memset(&unused, 0, sizeof(unused));
-        return tc_launch(ctx, 2, grid, smem, unused, tm_a, tm_bh, p);
+        return tc_launch(ctx, true, grid, smem, tm_a, tm_b, p);
       }
     }
     // not eligible after all: restore the standard geometry
@@ -696,23 +642,16 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   CUtensorMap tm_b;
   memset(&tm_as, 0, sizeof(tm_as));
   for (int v = 0; v < 4; ++v) {
-    int vv = v < nviews ? v : 0;
+    int vv = v < c.nviews ? v : 0;
     // stride-2 phase views of an odd-sized tensor differ in extent: rows 2r+a < H  =>  (H - a + 1) / 2 rows in phase a
     int vh = h, vw = w;
-    if (nviews == 4 && view_phase_of) { vh = (view_phase_of[0] - (vv >> 1) + 1) / 2; vw = (view_phase_of[1] - (vv & 1) + 1) / 2; }
+    if (c.nviews == 4 && c.phase_h > 0) { vh = (c.phase_h - (vv >> 1) + 1) / 2; vw = (c.phase_w - (vv & 1) + 1) / 2; }
     if (vh < 1 || vw < 1) { vh = h; vw = w; vv = 0; }
-    if (!make_act_map(&tm_as.m[v], in + view_off[vv], kdim, vw, vh, n, in_sw, in_sh, in_sn, p.bw, p.bh, p.bni))
+    if (!make_act_map(&tm_as.m[v], c.in + c.view_off[vv], kdim, vw, vh, n, c.in_sw, c.in_sh, c.in_sn, p.bw, p.bh, p.bni))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A) failed%s", "cgan_conv_tc");
   }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
-    cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
-    cuuint32_t box[3] = {TC_BK, (cuuint32_t)p.bn, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&tm_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
-  }
+  if (!make_weight_map(&tm_b, wt, kdim_pad, ncols_pad, c.taps_total, p.bn))
+    return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
 
   // Pixel tiles per CTA: with mt = 2 the weight tile is fetched once for 256 pixels, which cuts the L2->SM bytes per MMA
   // by a third; the accumulators (mt x bn columns) must fit the consumer registers, so only for bn <= 128, and only when
@@ -723,7 +662,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   p.tiles_total = (int)tiles_total;
   p.mt = 1;
   if (ctx->tc_mt_max >= 2 && 2 * p.bn <= TC_ACC_COLS && tiles_total * ncol_tiles * p.nphases >= 4ll * ctx->num_sms &&
-      (wimg_stride == 0 || (p.tiles_w * p.tiles_h) % 2 == 0))
+      (c.wimg_stride == 0 || (p.tiles_w * p.tiles_h) % 2 == 0))
     p.mt = 2;
   const bool two_ctas = p.mt * p.bn <= 128;
   const size_t stage_bytes = (size_t)p.mt * TC_A_BYTES + (size_t)p.bn * TC_BK * 4;
@@ -733,18 +672,5 @@ int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* vi
   p.vec2 = tc_vec2(p);
   size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/;
   dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles, (unsigned)p.nphases);
-  // CGAN_OPT_TC_PAIR: neighbouring CTAs run as two-CTA clusters that share each weight tile through TMA multicast
-  if (ctx->tc_pair && wimg_stride == 0 && grid.x >= 2) {
-    CUtensorMap tm_bh;
-    cuuint64_t dims[3] = {(cuuint64_t)kdim_pad, (cuuint64_t)ncols_pad, (cuuint64_t)taps_total};
-    cuuint64_t strides[2] = {(cuuint64_t)kdim_pad * 4, (cuuint64_t)ncols_pad * kdim_pad * 4};
-    cuuint32_t box[3] = {TC_BK, (cuuint32_t)(p.bn / 2), 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    if (enc(&tm_bh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, wt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B half) failed%s", "cgan_conv_tc");
-    grid.x = (grid.x + 1) / 2 * 2;
-    return tc_launch(ctx, 1, grid, smem, tm_as, tm_bh, tm_bh, p);
-  }
-  return tc_launch(ctx, 0, grid, smem, tm_as, tm_b, tm_b, p);
+  return tc_launch(ctx, false, grid, smem, tm_as, tm_b, p);
 }

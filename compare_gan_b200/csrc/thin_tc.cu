@@ -19,12 +19,6 @@
 // accumulation — the same as every other tensor-core contraction of math_mode 1 (CGAN_PATH_TCGEN05_TF32).
 #include "common.cuh"
 
-int cgan_conv_tc(cgan_ctx* ctx, const float* in, int nviews, const long long* view_off, long long in_sw, long long in_sh,
-                 long long in_sn, int n, int h, int w, int gh, int gw, int kdim, const float* wsrc, int taps_total,
-                 int transpose_w, int ncols, int ntaps, const int* off_h, const int* off_w, const int* wtap, const int* amap,
-                 const float* bias, float* out, long long s_n, long long s_h, long long s_w, long long base, int relu,
-                 const int* view_phase_of, int wimg_stride, const TcExtra* ex);
-bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols);
 bool cgan_wgrad_tc_geometry_ok(int n, int h, int w);
 int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw, int x_tf32, int dy_tf32);
 
@@ -137,17 +131,25 @@ inline int ew_blocks(cgan_ctx* ctx, long long n) {
   return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
-// forward taps of the convolution d: tap (kh, kw) reads the input at output*stride + (kh - pad_t, kw - pad_l)
-inline void taps_forward(const cgan_conv_desc* d, int c, TapList* t) {
-  t->ntaps = d->kh * d->kw; t->c = c; t->k = t->ntaps * c;
-  for (int kh = 0; kh < d->kh; ++kh)
-    for (int kw = 0; kw < d->kw; ++kw) { t->off_h[kh * d->kw + kw] = kh - d->pad_t; t->off_w[kh * d->kw + kw] = kw - d->pad_l; }
+// direct taps of the convolution d over C channels: sign +1, the forward taps (tap (kh, kw) reads the input at
+// output*stride + (kh - pad_t, kw - pad_l)); -1, the adjoint taps (stride 1: input pixel ih receives tap kh from output row
+// ih + pad_t - kh)
+inline void tap_list(const cgan_conv_desc* d, int sign, int c, TapList* t) {
+  ConvTaps ct;
+  conv_taps(d, sign, TAP_DIRECT, &ct);
+  t->ntaps = ct.ntaps; t->c = c; t->k = ct.ntaps * c;
+  for (int i = 0; i < ct.ntaps; ++i) { t->off_h[i] = ct.off_h[i]; t->off_w[i] = ct.off_w[i]; }
 }
-// adjoint taps (stride 1): input pixel ih receives tap kh from output row ih + pad_t - kh
-inline void taps_adjoint(const cgan_conv_desc* d, int c, TapList* t) {
-  t->ntaps = d->kh * d->kw; t->c = c; t->k = t->ntaps * c;
-  for (int kh = 0; kh < d->kh; ++kh)
-    for (int kw = 0; kw < d->kw; ++kw) { t->off_h[kh * d->kw + kw] = d->pad_t - kh; t->off_w[kh * d->kw + kw] = d->pad_l - kw; }
+
+// y = x W over a dense NHWC [n, h, w, kdim] operand: a 1x1 convolution on the tensor cores
+inline TcConv tc_gemm(const float* x, int n, int h, int w, int kdim, const float* wsrc, int transpose_w, int ncols, float* y,
+                      int ldy) {
+  TcConv c = {};
+  tc_in_dense(&c, x, n, h, w, kdim);
+  c.wsrc = wsrc; c.taps_total = 1; c.transpose_w = transpose_w; c.ncols = ncols;
+  c.taps.ntaps = 1;
+  tc_out_dense(&c, y, h, w, ldy);
+  return c;
 }
 
 inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -163,17 +165,6 @@ inline int tt_workspace(cgan_ctx* ctx, long long pixels, float** big, float** sm
   *small0 = reinterpret_cast<float*>(b + big_bytes);
   *small1 = reinterpret_cast<float*>(b + big_bytes + (64u << 10));
   return CGAN_OK;
-}
-
-inline TcExtra extra_from(const cgan_conv_epilogue* ep, int a_prerounded) {
-  TcExtra ex;
-  memset(&ex, 0, sizeof(ex));
-  ex.a_prerounded = a_prerounded;
-  if (ep) {
-    ex.round_out = (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0;
-    ex.residual = ep->residual; ex.mask = ep->mask; ex.mask_leak = ep->mask_leak;
-  }
-  return ex;
 }
 
 inline bool common_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
@@ -198,21 +189,16 @@ int cgan_thin_tc_fwd_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x,
   int rc = tt_workspace(ctx, pixels, &pt, &s0, &s1);
   if (rc) return rc;
   TapList t;
-  taps_forward(d, d->cin, &t);
+  tap_list(d, 1, d->cin, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, x, t, d->n, d->oh, d->ow, d->h, d->w, d->stride);
   CGAN_LAUNCHED(ctx);
   // HWIO flattened is [K = kh*kw*cin][cout]: padded to 32 rows so that the GEMM sees plain 32-channel operands
   pad_rows_kernel<<<cdiv((long long)TT_K * d->cout, 256), 256, 0, ctx->stream>>>(s0, w, t.k, TT_K, d->cout);
   CGAN_LAUNCHED(ctx);
-  const int ldy = (ep && ep->ldy) ? ep->ldy : d->cout;
-  const long long zero = 0;
-  const int o0 = 0;
-  TcExtra ex = extra_from(ep, 1);
   // y = P W: a 1x1 convolution over the 32-channel patch tensor
-  return cgan_conv_tc(ctx, pt, 1, &zero, TT_K, (long long)d->ow * TT_K, (long long)d->oh * d->ow * TT_K, d->n, d->oh, d->ow, d->oh,
-                      d->ow, TT_K, s0, 1, 1, d->cout, 1, &o0, &o0, &o0, nullptr, ep ? ep->bias : nullptr, y,
-                      (long long)d->oh * d->ow * ldy, (long long)d->ow * ldy, ldy, 0, (ep && (ep->flags & CGAN_CONV_RELU)) ? 1 : 0,
-                      nullptr, 0, &ex);
+  TcConv c = tc_gemm(pt, d->n, d->oh, d->ow, TT_K, s0, 1, d->cout, y, (ep && ep->ldy) ? ep->ldy : d->cout);
+  tc_set_epilogue(&c, ep, true);
+  return cgan_conv_tc(ctx, c);
 }
 
 bool cgan_thin_tc_wgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
@@ -225,7 +211,7 @@ int cgan_thin_tc_wgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   int rc = tt_workspace(ctx, pixels, &pt, &s0, &s1);
   if (rc) return rc;
   TapList t;
-  taps_forward(d, d->cin, &t);
+  tap_list(d, 1, d->cin, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, x, t, d->n, d->oh, d->ow, d->h, d->w, d->stride);
   CGAN_LAUNCHED(ctx);
   cgan_conv_desc g;          // dW32[32][cout] = P^T dy: the filter gradient of a 1x1 convolution 32 -> cout on the output grid
@@ -248,19 +234,16 @@ int cgan_thin_tc_dgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   int rc = tt_workspace(ctx, pixels, &tt, &s0, &s1);
   if (rc) return rc;
   TapList t;
-  taps_adjoint(d, d->cin, &t);
-  const long long zero = 0;
-  const int o0 = 0;
-  TcExtra ex = extra_from(nullptr, (ep && (ep->flags & CGAN_CONV_IN_TF32)) ? 1 : 0);
+  tap_list(d, -1, d->cin, &t);
   // T[p][tap*cin + ci] = sum_co dy[p][co] w[tap][ci][co]: HWIO flattened is [ncols = K][kdim = cout]
-  rc = cgan_conv_tc(ctx, dy, 1, &zero, d->cout, (long long)d->ow * d->cout, (long long)d->oh * d->ow * d->cout, d->n, d->oh, d->ow,
-                    d->oh, d->ow, d->cout, w, 1, 0, t.k, 1, &o0, &o0, &o0, nullptr, nullptr, tt, (long long)d->oh * d->ow * TT_K,
-                    (long long)d->ow * TT_K, TT_K, 0, 0, nullptr, 0, &ex);
+  TcConv c = tc_gemm(dy, d->n, d->oh, d->ow, d->cout, w, 0, t.k, tt, TT_K);
+  tc_set_epilogue(&c, nullptr, ep && (ep->flags & CGAN_CONV_IN_TF32));
+  rc = cgan_conv_tc(ctx, c);
   if (rc) return rc;
   shift_add_kernel<<<ew_blocks(ctx, (long long)d->n * d->h * d->w), 256, 0, ctx->stream>>>(dx, tt, ep ? ep->bias : nullptr, t, d->n,
                                                                                            d->h, d->w, d->oh, d->ow, 0);
   CGAN_LAUNCHED(ctx);
-  if (ep && (ep->residual || ep->mask || (ep->flags & (CGAN_CONV_RELU | CGAN_CONV_ROUND_OUT))))
+  if (ep_needs_post(ep, false))
     return cgan_conv_post_epilogue(ctx, dx, (int64_t)d->n * d->h * d->w, d->cin, d->cin, ep->residual, ep->mask, ep->mask_leak,
                                    (ep->flags & CGAN_CONV_RELU) ? 1 : 0, (ep->flags & CGAN_CONV_ROUND_OUT) ? 1 : 0);
   return CGAN_OK;
@@ -279,18 +262,15 @@ int cgan_thin_tc_fwd_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x
   int rc = tt_workspace(ctx, pixels, &tt, &wp, &s1);
   if (rc) return rc;
   TapList t;
-  taps_forward(d, d->cout, &t);
+  tap_list(d, 1, d->cout, &t);
   wcols_from_hwio_kernel<<<cdiv((long long)d->cin * TT_K, 256), 256, 0, ctx->stream>>>(wp, w, t.ntaps, d->cin, d->cout, TT_K);
   CGAN_LAUNCHED(ctx);
-  const long long zero = 0;
-  const int o0 = 0;
-  TcExtra ex = extra_from(nullptr, (ep && (ep->flags & CGAN_CONV_IN_TF32)) ? 1 : 0);
   // T[p][tap*cout + co] = sum_ci x[p][ci] w[tap][ci][co]: every tap's contribution at the INPUT pixel, all taps in one GEMM
-  rc = cgan_conv_tc(ctx, x, 1, &zero, d->cin, (long long)d->w * d->cin, (long long)d->h * d->w * d->cin, d->n, d->h, d->w, d->h, d->w,
-                    d->cin, wp, 1, 1, TT_K, 1, &o0, &o0, &o0, nullptr, nullptr, tt, (long long)d->h * d->w * TT_K, (long long)d->w * TT_K,
-                    TT_K, 0, 0, nullptr, 0, &ex);
+  TcConv c = tc_gemm(x, d->n, d->h, d->w, d->cin, wp, 1, TT_K, tt, TT_K);
+  tc_set_epilogue(&c, nullptr, ep && (ep->flags & CGAN_CONV_IN_TF32));
+  rc = cgan_conv_tc(ctx, c);
   if (rc) return rc;
-  const bool post = ep && (ep->residual || ep->mask || (ep->flags & CGAN_CONV_ROUND_OUT));
+  const bool post = ep_needs_post(ep, true);
   const int relu = (ep && (ep->flags & CGAN_CONV_RELU)) ? 1 : 0;
   shift_add_kernel<<<ew_blocks(ctx, pixels), 256, 0, ctx->stream>>>(y, tt, ep ? ep->bias : nullptr, t, d->n, d->oh, d->ow, d->h, d->w,
                                                                    post ? 0 : relu);
@@ -308,18 +288,15 @@ int cgan_thin_tc_dgrad_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float*
   int rc = tt_workspace(ctx, pixels, &pt, &wp, &s1);
   if (rc) return rc;
   TapList t;
-  taps_adjoint(d, d->cout, &t);
+  tap_list(d, -1, d->cout, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, dy, t, d->n, d->h, d->w, d->oh, d->ow, 1);
   CGAN_LAUNCHED(ctx);
   wcols_from_hwio_kernel<<<cdiv((long long)d->cin * TT_K, 256), 256, 0, ctx->stream>>>(wp, w, t.ntaps, d->cin, d->cout, TT_K);
   CGAN_LAUNCHED(ctx);
-  const long long zero = 0;
-  const int o0 = 0;
-  TcExtra ex = extra_from(ep, 1);
   // dx[p][ci] = sum_m P[p][m] W'[ci][m]: W' [ncols = cin][kdim = 32], columns >= K zero
-  return cgan_conv_tc(ctx, pt, 1, &zero, TT_K, (long long)d->w * TT_K, (long long)d->h * d->w * TT_K, d->n, d->h, d->w, d->h, d->w, TT_K,
-                      wp, 1, 0, d->cin, 1, &o0, &o0, &o0, nullptr, ep ? ep->bias : nullptr, dx, (long long)d->h * d->w * d->cin,
-                      (long long)d->w * d->cin, d->cin, 0, (ep && (ep->flags & CGAN_CONV_RELU)) ? 1 : 0, nullptr, 0, &ex);
+  TcConv c = tc_gemm(pt, d->n, d->h, d->w, TT_K, wp, 0, d->cin, dx, d->cin);
+  tc_set_epilogue(&c, ep, true);
+  return cgan_conv_tc(ctx, c);
 }
 
 bool cgan_thin_tc_wgrad_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
@@ -333,7 +310,7 @@ int cgan_thin_tc_wgrad_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float*
   int rc = tt_workspace(ctx, pixels, &pt, &s0, &dwp);
   if (rc) return rc;
   TapList t;
-  taps_adjoint(d, d->cout, &t);
+  tap_list(d, -1, d->cout, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, dy, t, d->n, d->h, d->w, d->oh, d->ow, 1);
   CGAN_LAUNCHED(ctx);
   cgan_conv_desc g;          // dW'[cin][32] = x^T P

@@ -291,25 +291,17 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const 
   p.co_tiles = (d->cout + p.bn - 1) / p.bn;
   p.cin = d->cin; p.cout = d->cout; p.taps_total = d->kh * d->kw;
   // taps: the pixel loop runs over a grid (i, j) of gh x gw cells: the input grid (stride 1, incl. zero-inserted
-  // inputs) or the output grid (stride 2); tap (kh,kw) pairs X view `amap` at [i+dh, j+dw] with dY view `bmap` at [i, j]
-  int nt = 0;
-  for (int kh = 0; kh < d->kh; ++kh)
-    for (int kw = 0; kw < d->kw; ++kw) {
-      p.amap[nt] = 0;
-      if (d->stride == 2) {
-        // output (i,j) reads input row 2i + kh - pad_t = 2(i + dh) + a: phase view a of X
-        int th = kh - d->pad_t, tw = kw - d->pad_l, a = th & 1, b = tw & 1;
-        p.off_h[nt] = (th - a) / 2; p.off_w[nt] = (tw - b) / 2; p.amap[nt] = a * 2 + b; p.bmap[nt] = 0;
-      } else if (!d->upsample) {
-        p.off_h[nt] = kh - d->pad_t; p.off_w[nt] = kw - d->pad_l; p.bmap[nt] = 0;
-      } else {
-        // output row 2i+a reads virtual row 2i+a+kh-pad_t, real only when even: a = (pad_t - kh) & 1, dh = (a+kh-pad_t)/2
-        int a = (d->pad_t - kh) & 1, b = (d->pad_l - kw) & 1;
-        p.off_h[nt] = (a + kh - d->pad_t) / 2; p.off_w[nt] = (b + kw - d->pad_l) / 2; p.bmap[nt] = a * 2 + b;
-      }
-      p.wtap[nt] = kh * d->kw + kw;
-      ++nt;
-    }
+  // inputs) or the output grid (stride 2); tap (kh,kw) pairs X view `amap` at [i+dh, j+dw] with dY view `bmap` at [i, j].
+  // Stride 2: output (i,j) reads input row 2i + kh - pad_t = 2(i + dh) + a, phase view a of X.  Zero-inserted input:
+  // output row 2i+a reads virtual row 2i+a+kh-pad_t, real only when even, from dY phase view a = (pad_t - kh) & 1.
+  ConvTaps t;
+  conv_taps(d, d->upsample ? -1 : 1, d->stride == 2 ? TAP_VIEW : d->upsample ? TAP_PHASE : TAP_DIRECT, &t);
+  const int nt = t.ntaps;
+  for (int i = 0; i < nt; ++i) {
+    p.off_h[i] = t.off_h[i]; p.off_w[i] = t.off_w[i]; p.wtap[i] = t.wtap[i];
+    p.amap[i] = d->upsample ? 0 : t.view[i];
+    p.bmap[i] = d->upsample ? t.view[i] : 0;
+  }
   p.ntaps = nt;
   // two (tap, ci-tile) units per CTA when they read the same dY view: dY is then fetched once per k-block for both
   const int units = p.ci_tiles * nt;

@@ -46,18 +46,12 @@ int64_t cgan_launch_count(cgan_ctx* ctx);
  *   CGAN_OPT_TC_HALO    (set/get) 3x3 stride-1 tensor-core convolutions fetch one (rows+2)-row activation box per kernel
  *                       column instead of one box per tap: 0 never, 1 where the operand is rounded in the kernel and there
  *                       are >= 256 output channels (default), 2 wherever the geometry allows.
- *   CGAN_OPT_TC_PAIR    (set/get) 1: the per-tap tensor-core convolutions run as two-CTA clusters that share each weight
- *                       tile through TMA multicast (same products in the same order); 0 (default): single CTAs, which
- *                       measured faster on an H100 (3x3 256->256 and 128->128 convs at 32x32).
- *   CGAN_OPT_TC_EPI     (set/get) accepted and reported; the epilogue stores straight from the accumulator fragments
- *                       (a lane quad covers 32 contiguous bytes of a row) for every value.
  *   CGAN_OPT_TC_THIN    (set/get) 1 (default): in math_mode 1 the image-side convolutions (<= 4 input or <= 4 output channels,
  *                       kh*kw*channels <= 32: every discriminator's first and every generator's last convolution, Inception's
  *                       stem) run as ONE 32-wide GEMM on the tensor-core kernels over a [pixels, 32] patch tensor (csrc/thin_tc.cu),
  *                       TF32 operands like every other tensor-core contraction; 0: the exact-fp32 streaming kernels (thin.cu).
  *   CGAN_OPT_LAST_PATH  (get) CGAN_PATH_* taken by the most recent conv2d_fwd / dgrad / wgrad / gemm_batched call. */
-enum { CGAN_OPT_TC_MT = 1, CGAN_OPT_LAST_PATH = 2, CGAN_OPT_TC_HALO = 3, CGAN_OPT_TC_PAIR = 4, CGAN_OPT_TC_EPI = 5,
-       CGAN_OPT_TC_THIN = 6 };
+enum { CGAN_OPT_TC_MT = 1, CGAN_OPT_LAST_PATH = 2, CGAN_OPT_TC_HALO = 3, CGAN_OPT_TC_THIN = 6 };
 /* CGAN_PATH_TCGEN05_TF32 keeps its name for ABI compatibility: the TF32 tensor-core (wgmma) path. */
 enum { CGAN_PATH_SIMT_FP32 = 0, CGAN_PATH_TCGEN05_TF32 = 1, CGAN_PATH_THIN_FP32 = 2 };
 int cgan_ctx_set_option(cgan_ctx* ctx, int key, int64_t value);
