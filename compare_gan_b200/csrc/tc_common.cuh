@@ -72,11 +72,16 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
   return (uint32_t)(row * 128 + ((((k >> 2) ^ row) & 7) << 4) + (k & 3) * 4);
 }
 
-// explicit shared-space 128-bit accesses: a pointer carved out of the dynamic smem buffer compiles to GENERIC LD/ST
-// LD.E.128 / ST.E.128; these are LDS.128 / STS.128
+// explicit shared-space accesses: a pointer carved out of the dynamic smem buffer compiles to GENERIC LD/ST
+// LD.E.128 / ST.E.128; these are LDS / LDS.128 / STS.128
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ float lds32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
   return v;
 }
 __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {

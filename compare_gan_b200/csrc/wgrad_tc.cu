@@ -9,7 +9,8 @@
 // each box = 32 rows x 128 B, unswizzled.  wgmma takes 32-bit operands only K-major, so the two consumer warpgroups
 // transpose both operands into 128B-swizzled K-major tiles (one 128-byte row of 32 pixels per channel), rounding them to
 // nearest TF32 on the way, into one of two transposed buffers; the TMA stage is released as soon as it has been read.
-// Four wgmma m64nNk8 per warpgroup (K = 8 pixels) consume a k-block; warpgroup g owns ci rows 64g..64g+63.
+// Four wgmma m64nNk8 per warpgroup (K = 8 pixels) consume a k-block; warpgroup g owns ci rows 64g..64g+63.  The
+// transposition of k-block kb + 1 runs while the MMAs of kb are in flight.
 // The pixel range is split across CTAs (split-K); partial tiles go to a workspace and are summed in a fixed order
 // (deterministic), replacing TF's Conv2DBackpropFilter.
 // A conv over a zero-inserted 2x-upsampled input (resnet_ops.py:35-56) is handled through four strided TMA views of dY
@@ -44,17 +45,29 @@ struct WgParams {
 
 struct BMaps { CUtensorMap m[4]; };
 
-// [32 pixels][rows] (unswizzled boxes of 32 channels, box g at g * WG_BOX) -> K-major swizzled [rows][32 pixels]
-__device__ __forceinline__ void wg_transpose(uint32_t dst, uint32_t src, int rows, bool round, int tid) {
-  const int groups = rows / 4;                        // float4 of 4 consecutive channels
-  for (int e = tid; e < groups * WG_P; e += 32 * WG_CWARPS) {
-    const int r = (e % groups) * 4, pix = e / groups;
-    float4 v = lds128(src + (r >> 5) * WG_BOX + pix * 128 + (r & 31) * 4);
-    if (round) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w); }
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r, pix)), "f"(v.x) : "memory");
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 1, pix)), "f"(v.y) : "memory");
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 2, pix)), "f"(v.z) : "memory");
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + 3, pix)), "f"(v.w) : "memory");
+// [32 pixels][ROWS] (unswizzled boxes of 32 channels, box b at b * WG_BOX) -> K-major swizzled [ROWS][32 pixels].
+// Consumer warp w (0..7) moves pixels 4w..4w+3 of every row, lane = channel within a box.  Each LDS.32 of a warp reads
+// one 128-byte pixel row of a box (one wavefront); each STS.128 writes 4 pixels into rows 32b..32b+31 at 16-byte chunk
+// (w ^ row) & 7, so every 8 consecutive rows take 8 distinct chunks and the warp's 512 bytes go out in 4 wavefronts,
+// the minimum.  Loads are issued four boxes at a time ahead of their stores.
+template <int ROWS>
+__device__ __forceinline__ void wg_transpose(uint32_t dst, uint32_t src, bool round, int warp, int lane) {
+  constexpr int NB = ROWS / 32;
+#pragma unroll
+  for (int b0 = 0; b0 < NB; b0 += 4) {
+    float4 v[4];
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      if (b0 + b >= NB) break;
+      const uint32_t s = src + (b0 + b) * WG_BOX + warp * 4 * 128 + lane * 4;
+      v[b] = make_float4(lds32(s), lds32(s + 128), lds32(s + 256), lds32(s + 384));
+    }
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      if (b0 + b >= NB) break;
+      if (round) { v[b].x = rna_tf32(v[b].x); v[b].y = rna_tf32(v[b].y); v[b].z = rna_tf32(v[b].z); v[b].w = rna_tf32(v[b].w); }
+      sts128(dst + sw128_offset((b0 + b) * 32 + lane, 4 * warp), v[b]);
+    }
   }
 }
 
@@ -88,7 +101,7 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);              // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[s], WG_CWARPS);      // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -127,8 +140,12 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   }
 
   // ===== consumer warpgroups =====
+  // k-block kb: transpose stage kb into buffer kb & 1 while this warpgroup's MMAs of kb - 1 (on the other buffer) run,
+  // then wait for those MMAs, then one CTA barrier, then issue the MMAs of kb.  Invariant: a warpgroup writes buffer
+  // kb & 1 only after the barrier of kb - 1, which both warpgroups reach only once their MMAs of kb - 2 (the last reads
+  // of that buffer) have retired; and the MMAs of kb start only after the barrier of kb, when both warpgroups' halves of
+  // the transposed tiles are written and made visible to the async proxy.
   const int wg = warp >> 2;
-  const int tid = threadIdx.x;                   // 0..255
   float acc[MT][BN / 2];
 #pragma unroll
   for (int u = 0; u < MT; ++u)
@@ -140,12 +157,14 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
     mbar_wait(&full_bar[stage], phase);
     const uint32_t s_addr = smem_u32(smem + stage * stage_bytes);
     const uint32_t t_addr = smem_u32(tbuf + (kb & 1) * stage_bytes);
-    // both warpgroups' MMAs that read this transposed buffer (k-block kb - 2) retired before the barrier of kb - 1
-    for (int i = 0; i < nu; ++i) wg_transpose(t_addr + i * WG_A_BYTES, s_addr + i * WG_A_BYTES, 128, p.round_a, tid);
-    wg_transpose(t_addr + a_bytes, s_addr + a_bytes, BN, p.round_b, tid);
+    for (int i = 0; i < nu; ++i) wg_transpose<128>(t_addr + i * WG_A_BYTES, s_addr + i * WG_A_BYTES, p.round_a, warp, lane);
+    wg_transpose<BN>(t_addr + a_bytes, s_addr + a_bytes, p.round_b, warp, lane);
+    // the warp's reads of the TMA stage are complete (their values are stored): release it to the producer
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
     fence_proxy_async();
+    wgmma_wait<0>();                              // this warpgroup's MMAs of kb - 1 retired
     named_bar(1, 32 * WG_CWARPS);
-    if ((tid & 127) == 0) mbar_arrive(&empty_bar[stage]);
 #pragma unroll
     for (int u = 0; u < MT; ++u)
 #pragma unroll
@@ -160,13 +179,13 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
                        make_desc(t_addr + a_bytes + k * 32));
     }
     wgmma_commit();
-    wgmma_wait<0>();
-#pragma unroll
-    for (int u = 0; u < MT; ++u)
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
   }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int u = 0; u < MT; ++u)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
   // epilogue: rows ci = m, m + 8 of each unit's tile, columns co0 + 8j + 2 (lane % 4) + {0, 1}
   const int c2 = (lane & 3) * 2;
   const bool vec2 = (p.cout & 1) == 0;
@@ -223,7 +242,9 @@ int pick_bn(int ncols) {
   return 0;
 }
 
-// TMA ring depth for a shared-memory budget (ring + the two transposed buffers); returns the dynamic smem size
+// TMA ring depth for a shared-memory budget (ring + the two transposed buffers; the barrier placement in the consumer
+// loop lets the transpose overlap the MMAs without a third one); returns the dynamic smem size.  A 48 KB stage (BN 256
+// with MT 1, or BN 128 with MT 2) gets a 2-deep ring and one CTA per SM; stages up to 24 KB fit two CTAs per SM.
 size_t wg_smem(size_t stage_bytes, size_t budget, int* stages) {
   long long s = (long long)(budget / stage_bytes) - 2;
   if (s > WG_MAX_STAGES) s = WG_MAX_STAGES;
