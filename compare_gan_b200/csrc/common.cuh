@@ -73,6 +73,22 @@ static inline int cgan_ws(cgan_ctx* ctx, size_t bytes, void** out) {
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// grid of 256-thread blocks for a grid-stride loop over n elements, at most 16 blocks per SM
+static inline int ew_grid(cgan_ctx* ctx, long long n) {
+  long long b = (n + 255) / 256;
+  long long cap = (long long)ctx->num_sms * 16;
+  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
+// round to the nearest TF32 value, ties away from zero
+__device__ __forceinline__ float rna_tf32(float x) {
+  uint32_t u;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+  return __uint_as_float(u);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -153,20 +169,39 @@ static inline bool conv_taps_by_phase(const cgan_conv_desc* d, int sign, ConvTap
   return true;
 }
 
-// ---- launch descriptor of the wgmma implicit-GEMM convolution (cgan_conv_tc, conv_tc.cu) ----------------------------
-//   out[base + n*s_n + y*s_h + x*s_w + col] = epilogue(sum_{tap, k} view[tap][n, y + off_h, x + off_w, k] * W[wtap][col][k])
-// for every output pixel (n, y, x), y < gh, x < gw.  Zero-initialise, then fill through the helpers below.
-struct TcConv {
-  // activation operand: `nviews` (1 or 4) views [n, h, w, kdim] of `in`, view v starting at in + view_off[v]
+// ---- activation operand of the wgmma kernels: `nviews` (1 or 4) NHWC views [n, h, w, ch] of `in` ---------------------
+struct TcView {
   const float* in;
   int nviews;
-  long long view_off[4];
-  long long in_sw, in_sh, in_sn;      // pixel strides (floats)
-  int n, h, w, kdim;
+  long long view_off[4];              // view v starts at in + view_off[v]
+  long long sw, sh, sn;               // pixel strides (floats)
+  int n, h, w, ch;
   int phase_h, phase_w;               // > 0: the four views are the parity phases of a phase_h x phase_w tensor
-  int in_tf32;                        // the operand already holds TF32-representable values: no rounding in shared memory
+  int tf32;                           // the operand already holds TF32-representable values: no rounding in shared memory
+};
+
+// dense NHWC operand [n, h, w, c]
+static inline void tc_in_dense(TcView* a, const float* x, int n, int h, int w, int ch) {
+  a->in = x; a->nviews = 1; a->view_off[0] = 0;
+  a->sw = ch; a->sh = (long long)w * ch; a->sn = (long long)h * w * ch;
+  a->n = n; a->h = h; a->w = w; a->ch = ch;
+}
+// dense NHWC [n, H, W, c] read through its four parity phases: view 2a + b holds the pixels (2i + a, 2j + b)
+static inline void tc_in_phases(TcView* a, const float* x, int n, int H, int W, int ch) {
+  a->in = x; a->nviews = 4;
+  for (int v = 0; v < 4; ++v) a->view_off[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
+  a->sw = 2ll * ch; a->sh = 2ll * W * ch; a->sn = (long long)H * W * ch;
+  a->n = n; a->h = (H + 1) / 2; a->w = (W + 1) / 2; a->ch = ch;
+  a->phase_h = H; a->phase_w = W;
+}
+
+// ---- launch descriptor of the wgmma implicit-GEMM convolution (cgan_conv_tc, conv_tc.cu) ----------------------------
+//   out[base + n*s_n + y*s_h + x*s_w + col] = epilogue(sum_{tap, k} a.view[tap][n, y + off_h, x + off_w, k] * W[wtap][col][k])
+// for every output pixel (n, y, x), y < gh, x < gw.  Zero-initialise, then fill through the helpers below.
+struct TcConv {
+  TcView a;                           // activation operand, k = its channels
   int gh, gw;                         // output pixel grid
-  // weights [taps_total][kdim][ncols] (transpose_w = 1) or [taps_total][ncols][kdim] (transpose_w = 0)
+  // weights [taps_total][a.ch][ncols] (transpose_w = 1) or [taps_total][ncols][a.ch] (transpose_w = 0)
   const float* wsrc;
   int taps_total, transpose_w, ncols;
   int wimg_stride;                    // != 0: batched GEMM, image i multiplies weight slice wtap + i * wimg_stride
@@ -184,20 +219,6 @@ struct TcConv {
   int relu, round_out;
 };
 
-// dense NHWC operand [n, h, w, c]
-static inline void tc_in_dense(TcConv* c, const float* x, int n, int h, int w, int ch) {
-  c->in = x; c->nviews = 1; c->view_off[0] = 0;
-  c->in_sw = ch; c->in_sh = (long long)w * ch; c->in_sn = (long long)h * w * ch;
-  c->n = n; c->h = h; c->w = w; c->kdim = ch;
-}
-// dense NHWC [n, H, W, c] read through its four parity phases: view 2a + b holds the pixels (2i + a, 2j + b)
-static inline void tc_in_phases(TcConv* c, const float* x, int n, int H, int W, int ch) {
-  c->in = x; c->nviews = 4;
-  for (int v = 0; v < 4; ++v) c->view_off[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
-  c->in_sw = 2ll * ch; c->in_sh = 2ll * W * ch; c->in_sn = (long long)H * W * ch;
-  c->n = n; c->h = (H + 1) / 2; c->w = (W + 1) / 2; c->kdim = ch;
-  c->phase_h = H; c->phase_w = W;
-}
 // dense NHWC output over an h x w grid, rows of `ld` floats
 static inline void tc_out_dense(TcConv* c, float* y, int h, int w, int ld) {
   c->out = y; c->gh = h; c->gw = w;
@@ -211,7 +232,7 @@ static inline void tc_out_phases(TcConv* c, float* y, int H, int W, int ch) {
 }
 // the whole epilogue of `ep` (null: none) and whether the activation operand is already TF32-rounded
 static inline void tc_set_epilogue(TcConv* c, const cgan_conv_epilogue* ep, bool in_tf32) {
-  c->in_tf32 = in_tf32 ? 1 : 0;
+  c->a.tf32 = in_tf32 ? 1 : 0;
   if (!ep) return;
   c->bias = ep->bias; c->residual = ep->residual; c->mask = ep->mask; c->mask_leak = ep->mask_leak;
   c->relu = (ep->flags & CGAN_CONV_RELU) ? 1 : 0;
@@ -224,16 +245,60 @@ static inline bool ep_needs_post(const cgan_conv_epilogue* ep, bool relu_fused) 
   return ep && (ep->residual || ep->mask || (ep->flags & CGAN_CONV_ROUND_OUT) || (!relu_fused && (ep->flags & CGAN_CONV_RELU)));
 }
 
+// ---- launch descriptor of the wgmma filter-gradient kernel (cgan_wgrad_tc, wgrad_tc.cu) -----------------------------
+//   dw[wtap][ci][co] = sum_{n, y < dy.h, x < dy.w}  x.view[ax][n, y + off_h, x + off_w, ci] * dy.view[by][n, y, x, co]
+// for every tap, with (ax, by) = (taps.view, 0), or (0, taps.view) when taps_view_dy: the pixel grid is that of dy's
+// views.  Zero-initialise, then fill.
+struct TcWgrad {
+  TcView x;              // 1 view, or the four stride-2 parity phases (each of the grid's size)
+  TcView dy;             // 1 view over the grid, or the four sub-pixel phases of the gradient of a zero-inserted input
+  ConvTaps taps;
+  int taps_view_dy;      // taps.view indexes dy's views (zero-inserted input) instead of x's (stride 2)
+  int taps_total;        // dw holds taps_total slices [x.ch][dy.ch]
+  float* dw;
+  int per_image;         // per-image A^T B (one tap): dw slice i sums over image n = i only, stored with no reduce pass
+};
+
 int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c);
 // geometry the tensor-core convolution accepts for a stride-1 contraction
 bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols);
+int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g);
+// the filter-gradient kernel's own limits (box geometry, channel tiles, taps, alignment); routing policy is the caller's
+bool cgan_wgrad_tc_fits(const TcWgrad& g);
 
 // internal (C++ linkage) entry points shared between translation units
+// gemm.cu
 int cgan_conv2d_fwd_simt(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const float* bias, float* y,
                          int relu, int ldy);
 int cgan_conv2d_dgrad_simt(cgan_ctx*, const cgan_conv_desc*, const float* dy, const float* w, float* dx);
+int cgan_conv2d_wgrad_simt(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw);
+int cgan_gemm_batched_simt(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float alpha, const float* a, int lda,
+                           int64_t sa, const float* b, int ldb, int64_t sb, float beta, float* c, int ldc, int64_t sc, int batch);
+// out[i] = sum_{z < splits} part[z * n + i], summed in the order z = 0, 1, ... (deterministic split-K)
+int cgan_splitk_reduce(cgan_ctx* ctx, float* out, const float* part, long long n, int splits);
+// pointwise.cu
 int cgan_conv_post_epilogue(cgan_ctx* ctx, float* y, int64_t rows, int c, int ld, const float* residual, const float* mask,
                             float mask_leak, int relu, int round_out);
 int cgan_upsample1x1_bias_phases(cgan_ctx* ctx, float* out, const float* bias, int n, int oh, int ow, int c);
-int cgan_gemm_batched_simt(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float alpha, const float* a, int lda,
-                           int64_t sa, const float* b, int ldb, int64_t sb, float beta, float* c, int ldc, int64_t sc, int batch);
+// thin.cu: exact-fp32 streaming kernels for image-side (<= 4 channel) convolutions
+bool cgan_fwd_thin_ok(const cgan_conv_desc* d);
+int cgan_fwd_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y, int relu,
+                  int ldy, int round_out);
+bool cgan_fwd_thin3_ok(const cgan_conv_desc* d);
+bool cgan_pw_thin_ok(const cgan_conv_desc* d);
+int cgan_fwd_pw_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y,
+                     const float* residual, int relu, int ldy, int round_out);
+bool cgan_wgrad_thin_ok(const cgan_conv_desc* d);
+int cgan_wgrad_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw);
+// thin_tc.cu: image-side convolutions through a 32-wide patch tensor on the tensor cores
+bool cgan_thin_tc_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
+bool cgan_thin_tc_wgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
+bool cgan_thin_tc_dgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
+bool cgan_thin_tc_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
+bool cgan_thin_tc_wgrad_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
+int cgan_thin_tc_fwd_cin(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const cgan_conv_epilogue* ep, float* y);
+int cgan_thin_tc_wgrad_cin(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* dy, int dy_tf32, float* dw);
+int cgan_thin_tc_dgrad_cin(cgan_ctx*, const cgan_conv_desc*, const float* dy, const float* w, const cgan_conv_epilogue* ep, float* dx);
+int cgan_thin_tc_fwd_cout(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const cgan_conv_epilogue* ep, float* y);
+int cgan_thin_tc_dgrad_cout(cgan_ctx*, const cgan_conv_desc*, const float* dy, const float* w, const cgan_conv_epilogue* ep, float* dx);
+int cgan_thin_tc_wgrad_cout(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* dy, int x_tf32, float* dw);

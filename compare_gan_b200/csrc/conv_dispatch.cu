@@ -2,39 +2,6 @@
 // tensor-core implicit GEMM (conv_tc.cu, math_mode 1) according to the context's math mode and the shape.
 #include "common.cuh"
 
-bool cgan_fwd_thin_ok(const cgan_conv_desc* d);
-int cgan_fwd_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y, int relu,
-                  int ldy, int round_out);
-bool cgan_fwd_thin3_ok(const cgan_conv_desc* d);
-bool cgan_pw_thin_ok(const cgan_conv_desc* d);
-int cgan_fwd_pw_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y,
-                     const float* residual, int relu, int ldy, int round_out);
-int cgan_wgrad_tc_batched(cgan_ctx* ctx, const float* a, const float* b, float* c, int batch, int h, int w, int k1, int k2);
-bool cgan_wgrad_tc_ok(const cgan_conv_desc* d);
-int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw, int x_tf32, int dy_tf32);
-int cgan_conv2d_wgrad_simt(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw);
-bool cgan_wgrad_thin_ok(const cgan_conv_desc* d);
-int cgan_wgrad_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw);
-
-// image-side convolutions (<= 4 input or output channels) through a 32-wide patch tensor on the tensor cores (thin_tc.cu)
-bool cgan_thin_tc_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
-bool cgan_thin_tc_wgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
-bool cgan_thin_tc_dgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
-bool cgan_thin_tc_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
-bool cgan_thin_tc_wgrad_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d);
-int cgan_thin_tc_fwd_cin(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const cgan_conv_epilogue* ep, float* y);
-int cgan_thin_tc_wgrad_cin(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* dy, int dy_tf32, float* dw);
-int cgan_thin_tc_dgrad_cin(cgan_ctx*, const cgan_conv_desc*, const float* dy, const float* w, const cgan_conv_epilogue* ep, float* dx);
-int cgan_thin_tc_fwd_cout(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* w, const cgan_conv_epilogue* ep, float* y);
-int cgan_thin_tc_dgrad_cout(cgan_ctx*, const cgan_conv_desc*, const float* dy, const float* w, const cgan_conv_epilogue* ep, float* dx);
-int cgan_thin_tc_wgrad_cout(cgan_ctx*, const cgan_conv_desc*, const float* x, const float* dy, int x_tf32, float* dw);
-
-namespace {
-
-inline bool al16p(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-}  // namespace
-
 int cgan_conv2d_fwd(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* w, const float* bias, float* y) {
   return cgan_conv2d_fwd_act(ctx, d, x, w, bias, 0, y);
 }
@@ -69,9 +36,9 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   CGAN_REQUIRE(ctx, ldy >= d->cout, "ldy must be >= cout");
   CGAN_REQUIRE(ctx, ldy == d->cout || !d->upsample, "strided output is not available with upsample");
   const bool ld_ok = ldy == d->cout || ldy % 4 == 0;      // the tensor-core epilogue stores rows of float2 pairs (a multiple of 4 keeps them aligned)
-  const bool ptr_ok = al16p(x) && al16p(y) && (!bias || al16p(bias)) && (!ep || ((!ep->residual || al16p(ep->residual)) &&
-                                                                                  (!ep->mask || al16p(ep->mask))));
-  if (ctx->tc_thin && ptr_ok && ld_ok && al16p(w) && !(d->kh == 1 && d->kw == 1)) {
+  const bool ptr_ok = al16(x) && al16(y) && (!bias || al16(bias)) && (!ep || ((!ep->residual || al16(ep->residual)) &&
+                                                                                  (!ep->mask || al16(ep->mask))));
+  if (ctx->tc_thin && ptr_ok && ld_ok && al16(w) && !(d->kh == 1 && d->kw == 1)) {
     if (cgan_thin_tc_cin_ok(ctx, d)) {
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
       return cgan_thin_tc_fwd_cin(ctx, d, x, w, ep, y);
@@ -82,7 +49,7 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
     }
   }
   TcConv c = {};
-  tc_in_dense(&c, x, d->n, d->h, d->w, d->cin);
+  tc_in_dense(&c.a, x, d->n, d->h, d->w, d->cin);
   c.wsrc = w; c.taps_total = d->kh * d->kw; c.transpose_w = 1; c.ncols = d->cout;
   // a 1x1 kernel over a zero-inserted input (BigGAN's up-sampling shortcut): phase (0,0) is a plain 1x1 conv written to the
   // even pixels, the other three phases are bias only
@@ -128,7 +95,7 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   if (ctx->math_mode == 1 && d->stride == 2 && !d->upsample && d->kh * d->kw <= 32 && d->h >= 2 && d->w >= 2 &&
       (d->oh - 1) * 2 + d->kh - d->pad_t <= d->h + d->kh && cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cin, d->cout) &&
       ptr_ok && ld_ok) {
-    tc_in_phases(&c, x, d->n, d->h, d->w, d->cin);
+    tc_in_phases(&c.a, x, d->n, d->h, d->w, d->cin);
     conv_taps(d, 1, TAP_VIEW, &c.taps);
     tc_out_dense(&c, y, d->oh, d->ow, ldy);
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
@@ -137,7 +104,7 @@ int cgan_conv2d_fwd_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, c
   // exact-fp32 paths: residual / mask / rounding are applied by one extra pointwise pass
   bool post = ep_needs_post(ep, true);
   int rc;
-  if (cgan_pw_thin_ok(d) && ptr_ok && al16p(w) && ldy % 4 == 0 && !(ep && ep->mask)) {
+  if (cgan_pw_thin_ok(d) && ptr_ok && al16(w) && ldy % 4 == 0 && !(ep && ep->mask)) {
     // pointwise conv over <= 4 channels: one streaming kernel with residual add, ReLU and rounding fused
     ctx->last_path = CGAN_PATH_THIN_FP32;
     return cgan_fwd_pw_thin(ctx, d, x, w, bias, y, ep ? ep->residual : nullptr, relu, ldy,
@@ -169,10 +136,10 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
   const float* bias = ep ? ep->bias : nullptr;          // tf.nn.conv2d_transpose + bias (arch_ops.py:588-592)
   const int relu = (ep && (ep->flags & CGAN_CONV_RELU)) ? 1 : 0;
   const bool dy_tf32 = ep && (ep->flags & CGAN_CONV_IN_TF32);
-  const bool ptr_ok = al16p(dy) && al16p(dx) && (!bias || al16p(bias)) &&
-                      (!ep || ((!ep->residual || al16p(ep->residual)) && (!ep->mask || al16p(ep->mask))));
+  const bool ptr_ok = al16(dy) && al16(dx) && (!bias || al16(bias)) &&
+                      (!ep || ((!ep->residual || al16(ep->residual)) && (!ep->mask || al16(ep->mask))));
   const bool geom = d->oh == (d->upsample ? 2 * d->h : d->h) && d->ow == (d->upsample ? 2 * d->w : d->w);
-  if (ctx->tc_thin && ptr_ok && al16p(w) && !(d->kh == 1 && d->kw == 1)) {
+  if (ctx->tc_thin && ptr_ok && al16(w) && !(d->kh == 1 && d->kw == 1)) {
     if (cgan_thin_tc_cout_ok(ctx, d)) {          // dy has <= 4 channels (the generator's image conv)
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
       return cgan_thin_tc_dgrad_cout(ctx, d, dy, w, ep, dx);
@@ -185,7 +152,7 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
   // dx[n,ih,iw,ci] = sum_{kh,kw,co} dy[n, oh, ow, co] * w[kh,kw,ci,co]: HWIO is already [tap][row=ci][k=co], i.e.
   // K-major for this contraction (no transpose).
   TcConv c = {};
-  tc_in_dense(&c, dy, d->n, d->oh, d->ow, d->cout);
+  tc_in_dense(&c.a, dy, d->n, d->oh, d->ow, d->cout);
   c.wsrc = w; c.taps_total = d->kh * d->kw; c.transpose_w = 0; c.ncols = d->cin;
   tc_set_epilogue(&c, ep, dy_tf32);
   if (ctx->math_mode == 1 && d->stride == 1 && d->kh * d->kw <= 32 && geom &&
@@ -199,7 +166,7 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
     // zero-inserted input: the real pixel ih sits at virtual row 2*ih; tap kh reaches output row oh = 2*ih + pad_t - kh,
     // i.e. sub-pixel phase a = (pad_t - kh) & 1 of dy at phase-row ih + (pad_t - kh - a)/2.  The four phases are four
     // strided TMA views of dy.
-    tc_in_phases(&c, dy, d->n, d->oh, d->ow, d->cout);
+    tc_in_phases(&c.a, dy, d->n, d->oh, d->ow, d->cout);
     conv_taps(d, -1, TAP_VIEW, &c.taps);
     return cgan_conv_tc(ctx, c);
   }
@@ -237,7 +204,7 @@ int cgan_conv2d_wgrad(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, co
 int cgan_conv2d_wgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, int flags, float* dw) {
   if (!ctx) return CGAN_ERR_ARG;
   CGAN_REQUIRE(ctx, d && x && dy && dw, "null pointer");
-  if (ctx->tc_thin && d->n > 0 && d->kh * d->kw > 1 && al16p(x) && al16p(dy) && al16p(dw)) {
+  if (ctx->tc_thin && d->n > 0 && d->kh * d->kw > 1 && al16(x) && al16(dy) && al16(dw)) {
     if (cgan_thin_tc_wgrad_cin_ok(ctx, d)) {
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
       return cgan_thin_tc_wgrad_cin(ctx, d, x, dy, (flags & CGAN_CONV_IN2_TF32) ? 1 : 0, dw);
@@ -251,9 +218,36 @@ int cgan_conv2d_wgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x,
     ctx->last_path = CGAN_PATH_THIN_FP32;
     return cgan_wgrad_thin(ctx, d, x, dy, dw);      // exact fp32 streaming kernels for 3-channel image-side layers
   }
-  if (ctx->math_mode == 1 && cgan_wgrad_tc_ok(d) && al16p(x) && al16p(dy) && al16p(dw)) {
-    ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-    return cgan_wgrad_tc(ctx, d, x, dy, dw, (flags & CGAN_CONV_IN_TF32) ? 1 : 0, (flags & CGAN_CONV_IN2_TF32) ? 1 : 0);
+  // The pixel loop runs over dy's grid: the input grid for stride 1 (also a zero-inserted input) and the output grid
+  // for stride 2.  Stride 2: output (i, j) reads input row 2i + kh - pad_t = 2(i + dh) + a, i.e. parity phase view a
+  // of X.  Zero-inserted input: output row 2i + a reads virtual row 2i + a + kh - pad_t, real only when even, from the
+  // dY sub-pixel phase a = (pad_t - kh) & 1.
+  if (ctx->math_mode == 1 && d->cin >= 64) {
+    TcWgrad g = {};
+    bool geom = false;
+    if (d->stride == 2) {
+      geom = !d->upsample && !(d->h & 1) && !(d->w & 1) && d->oh == d->h / 2 && d->ow == d->w / 2 &&
+             conv_taps(d, 1, TAP_VIEW, &g.taps);
+      tc_in_phases(&g.x, x, d->n, d->h, d->w, d->cin);
+      tc_in_dense(&g.dy, dy, d->n, d->oh, d->ow, d->cout);
+    } else if (d->stride == 1 && d->upsample) {
+      geom = d->oh == 2 * d->h && d->ow == 2 * d->w && conv_taps(d, -1, TAP_PHASE, &g.taps);
+      g.taps_view_dy = 1;
+      tc_in_dense(&g.x, x, d->n, d->h, d->w, d->cin);
+      tc_in_phases(&g.dy, dy, d->n, d->oh, d->ow, d->cout);
+    } else if (d->stride == 1) {
+      geom = d->oh == d->h && d->ow == d->w && conv_taps(d, 1, TAP_DIRECT, &g.taps);
+      tc_in_dense(&g.x, x, d->n, d->h, d->w, d->cin);
+      tc_in_dense(&g.dy, dy, d->n, d->oh, d->ow, d->cout);
+    }
+    g.x.tf32 = (flags & CGAN_CONV_IN_TF32) ? 1 : 0;
+    g.dy.tf32 = (flags & CGAN_CONV_IN2_TF32) ? 1 : 0;
+    g.taps_total = d->kh * d->kw;
+    g.dw = dw;
+    if (geom && cgan_wgrad_tc_fits(g)) {
+      ctx->last_path = CGAN_PATH_TCGEN05_TF32;
+      return cgan_wgrad_tc(ctx, g);
+    }
   }
   ctx->last_path = CGAN_PATH_SIMT_FP32;
   return cgan_conv2d_wgrad_simt(ctx, d, x, dy, dw);
@@ -282,7 +276,7 @@ int cgan_gemm_batched(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float 
     const bool nn = !tb && ldb == n && sb == (int64_t)k * n;       // B[i] stored [k, n]  (transposed by the prep kernel)
     if (nt || nn) {
       TcConv g = {};
-      tc_in_dense(&g, a, batch, h, w, k);
+      tc_in_dense(&g.a, a, batch, h, w, k);
       g.wsrc = b; g.taps_total = batch; g.transpose_w = nn ? 1 : 0; g.ncols = n; g.wimg_stride = 1;
       g.taps.ntaps = 1;                // one tap at offset 0: image i multiplies weight slice i
       tc_out_dense(&g, c, h, w, n);
@@ -291,10 +285,19 @@ int cgan_gemm_batched(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float 
     }
   }
   if (ctx->math_mode == 1 && plain && ta && !tb && rows_as_grid(k, &h, &w) && lda == m && sa == (int64_t)k * m && ldb == n &&
-      sb == (int64_t)k * n && ldc == n && sc == (int64_t)m * n && m % 32 == 0 && m >= 64 && n % 4 == 0 && n <= 256 && k % 32 == 0) {
+      sb == (int64_t)k * n && ldc == n && sc == (int64_t)m * n && m >= 64 && n <= 256) {
     // C[i] = A[i]^T * B[i]: the reduction runs over the rows (pixels) -> the filter-gradient kernel, one image per CTA row
-    ctx->last_path = CGAN_PATH_TCGEN05_TF32;
-    return cgan_wgrad_tc_batched(ctx, a, b, c, batch, h, w, m, n);
+    TcWgrad g = {};
+    tc_in_dense(&g.x, a, batch, h, w, m);
+    tc_in_dense(&g.dy, b, batch, h, w, n);
+    g.taps.ntaps = 1;                    // one tap at offset 0
+    g.taps_total = 1;
+    g.dw = c;
+    g.per_image = 1;
+    if (cgan_wgrad_tc_fits(g)) {
+      ctx->last_path = CGAN_PATH_TCGEN05_TF32;
+      return cgan_wgrad_tc(ctx, g);
+    }
   }
   ctx->last_path = CGAN_PATH_SIMT_FP32;
   return cgan_gemm_batched_simt(ctx, ta, tb, m, n, k, alpha, a, lda, sa, b, ldb, sb, beta, c, ldc, sc, batch);

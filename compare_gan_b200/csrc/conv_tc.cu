@@ -450,7 +450,7 @@ int prep_weights(cgan_ctx* ctx, const TcConv& c, int kdim_pad, int ncols_pad, fl
   float* wt = reinterpret_cast<float*>(ws);
   long long tot = (long long)c.taps_total * ncols_pad * kdim_pad;
   long long blocks = (tot + 255) / 256, cap = (long long)ctx->num_sms * 8;
-  wprep_kernel<<<(int)(blocks > cap ? cap : blocks), 256, 0, ctx->stream>>>(wt, c.wsrc, c.taps_total, c.ncols, ncols_pad, c.kdim,
+  wprep_kernel<<<(int)(blocks > cap ? cap : blocks), 256, 0, ctx->stream>>>(wt, c.wsrc, c.taps_total, c.ncols, ncols_pad, c.a.ch,
                                                                              kdim_pad, c.transpose_w);
   CGAN_LAUNCHED(ctx);
   *out = wt;
@@ -512,8 +512,8 @@ bool cgan_tc_shape_ok(int n, int h, int w, int kdim, int ncols) {
 int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   if (!get_encode()) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled unavailable%s", "cgan_conv_tc");
   const ConvTaps& tp = c.taps;
-  if (tp.ntaps > TC_MAX_TAPS || c.nviews > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: too many taps/views%s", "cgan_conv_tc");
-  const int n = c.n, h = c.h, w = c.w, kdim = c.kdim, gh = c.gh, gw = c.gw, ntaps = tp.ntaps;
+  if (tp.ntaps > TC_MAX_TAPS || c.a.nviews > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: too many taps/views%s", "cgan_conv_tc");
+  const int n = c.a.n, h = c.a.h, w = c.a.w, kdim = c.a.ch, gh = c.gh, gw = c.gw, ntaps = tp.ntaps;
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.ntaps = ntaps;
@@ -529,7 +529,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   p.rows_used = p.bw * p.bh * p.bni;
   p.img_n = n; p.img_h = gh; p.img_w = gw;
   p.relu = c.relu;
-  p.round_a = c.in_tf32 ? 0 : 1;
+  p.round_a = c.a.tf32 ? 0 : 1;
   p.round_out = c.round_out; p.residual = c.residual; p.mask = c.mask; p.mask_leak = c.mask_leak;
   p.nphases = 1;
   p.ph_tap0[0] = 0; p.ph_tap0[1] = ntaps;
@@ -559,7 +559,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   // (bh+2)/bh per chunk); a pre-rounded operand streams through the per-tap kernel.  CGAN_OPT_TC_HALO = 2 forces it
   // everywhere (tests).
   const bool halo_wanted = ctx->tc_halo == 2 || (ctx->tc_halo == 1 && p.round_a && ncols_pad >= 256);
-  if (halo_wanted && p.nphases == 1 && c.nviews == 1 && c.wimg_stride == 0 && ntaps == 9 && gh == h && gw == w) {
+  if (halo_wanted && p.nphases == 1 && c.a.nviews == 1 && c.wimg_stride == 0 && ntaps == 9 && gh == h && gw == w) {
     int hbw = 0, hbh = 0;
     if (w % 32 == 0) { hbw = 32; hbh = 4; } else if (w == 16) { hbw = 16; hbh = 8; }
     // group the taps by horizontal offset; each group must be three vertically consecutive taps
@@ -621,7 +621,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
         AMaps tm_a;
         CUtensorMap tm_b;
         memset(&tm_a, 0, sizeof(tm_a));
-        if (!make_act_map(&tm_a.m[0], c.in + c.view_off[0], kdim, w, h, n, c.in_sw, c.in_sh, c.in_sn, hbw, hbh + 2, 1))
+        if (!make_act_map(&tm_a.m[0], c.a.in + c.a.view_off[0], kdim, w, h, n, c.a.sw, c.a.sh, c.a.sn, hbw, hbh + 2, 1))
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A halo) failed%s", "cgan_conv_tc");
         if (!make_weight_map(&tm_b, wt, kdim_pad, ncols_pad, c.taps_total, p.bn))
           return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
@@ -641,15 +641,9 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   AMaps tm_as;
   CUtensorMap tm_b;
   memset(&tm_as, 0, sizeof(tm_as));
-  for (int v = 0; v < 4; ++v) {
-    int vv = v < c.nviews ? v : 0;
-    // stride-2 phase views of an odd-sized tensor differ in extent: rows 2r+a < H  =>  (H - a + 1) / 2 rows in phase a
-    int vh = h, vw = w;
-    if (c.nviews == 4 && c.phase_h > 0) { vh = (c.phase_h - (vv >> 1) + 1) / 2; vw = (c.phase_w - (vv & 1) + 1) / 2; }
-    if (vh < 1 || vw < 1) { vh = h; vw = w; vv = 0; }
-    if (!make_act_map(&tm_as.m[v], c.in + c.view_off[vv], kdim, vw, vh, n, c.in_sw, c.in_sh, c.in_sn, p.bw, p.bh, p.bni))
+  for (int v = 0; v < 4; ++v)
+    if (!make_view_map(&tm_as.m[v], c.a, v, p.bw, p.bh, p.bni))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(A) failed%s", "cgan_conv_tc");
-  }
   if (!make_weight_map(&tm_b, wt, kdim_pad, ncols_pad, c.taps_total, p.bn))
     return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
 

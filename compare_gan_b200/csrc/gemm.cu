@@ -342,8 +342,6 @@ int launch(cgan_ctx* ctx, const GP& p, int gz) {
   return CGAN_OK;
 }
 
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 int check_desc(cgan_ctx* ctx, const cgan_conv_desc* d) {
   CGAN_REQUIRE(ctx, d != nullptr, "null descriptor");
   CGAN_REQUIRE(ctx, d->n > 0 && d->h > 0 && d->w > 0 && d->cin > 0 && d->cout > 0, "non-positive tensor dims");
@@ -432,7 +430,11 @@ int cgan_conv2d_wgrad_simt(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   p.C = reinterpret_cast<float*>(ws);
   rc = launch<M_WGRAD, false, false>(ctx, p, splits);
   if (rc) return rc;
-  splitk_reduce_kernel<<<cdiv(mn, 256), 256, 0, ctx->stream>>>(dw, p.C, mn, splits);
+  return cgan_splitk_reduce(ctx, dw, p.C, mn, splits);
+}
+
+int cgan_splitk_reduce(cgan_ctx* ctx, float* out, const float* part, long long n, int splits) {
+  splitk_reduce_kernel<<<cdiv(n, 256), 256, 0, ctx->stream>>>(out, part, n, splits);
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }

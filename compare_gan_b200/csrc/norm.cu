@@ -211,12 +211,6 @@ __global__ void bn_accu_counter_kernel(float* ac, const float* upd) {
   if (*upd == 1.0f) *ac += 1.0f;
 }
 
-__device__ __forceinline__ float rna_tf32n(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-
 // act: bit 0 = ReLU, CGAN_ACT_ROUND_TF32 = store TF32-rounded values
 __global__ void bn_apply_kernel(float* __restrict__ y, const float* __restrict__ x, long long total, int C,
                                 long long rows_per_sample, const float* __restrict__ mean_var, float eps,
@@ -232,7 +226,7 @@ __global__ void bn_apply_kernel(float* __restrict__ y, const float* __restrict__
     if (gamma) v *= gamma[pidx];
     if (beta) v += beta[pidx];
     if (relu) v = fmaxf(v, 0.f);
-    y[i] = rnd ? rna_tf32n(v) : v;
+    y[i] = rnd ? rna_tf32(v) : v;
   }
 }
 
@@ -255,7 +249,7 @@ __global__ void bn_apply_v4_kernel(float4* __restrict__ y, const float4* __restr
     if (gamma) { const float4 g = *reinterpret_cast<const float4*>(gamma + pidx); v.x *= g.x; v.y *= g.y; v.z *= g.z; v.w *= g.w; }
     if (beta) { const float4 b = *reinterpret_cast<const float4*>(beta + pidx); v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w; }
     if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-    if (rnd) { v.x = rna_tf32n(v.x); v.y = rna_tf32n(v.y); v.z = rna_tf32n(v.z); v.w = rna_tf32n(v.w); }
+    if (rnd) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w); }
     y[i] = v;
   }
 }
@@ -288,7 +282,7 @@ __global__ void bn_bwd_apply_kernel(float* __restrict__ dx, const float* __restr
     float g = gamma ? gamma[cond ? (r / rows_per_sample) * C + c : c] : 1.0f;
     float dxh = dy[i] * g;
     float v = inv * (dxh - sums[c] * inv_count - xh * sums[C + c] * inv_count);
-    dx[i] = rnd ? rna_tf32n(v) : v;
+    dx[i] = rnd ? rna_tf32(v) : v;
   }
 }
 
@@ -324,7 +318,7 @@ __global__ void bn_bwd_apply_v4_kernel(float4* __restrict__ dx, const float4* __
       const float inv = 1.0f / sqrtf(vv.w + eps), xh = (xv.w - m.w) * inv;
       o.w = inv * (gy.w * g.w - s1.w * inv_count - xh * s2.w * inv_count);
     }
-    if (rnd) { o.x = rna_tf32n(o.x); o.y = rna_tf32n(o.y); o.z = rna_tf32n(o.z); o.w = rna_tf32n(o.w); }
+    if (rnd) { o.x = rna_tf32(o.x); o.y = rna_tf32(o.y); o.z = rna_tf32(o.z); o.w = rna_tf32(o.w); }
     dx[i] = o;
   }
 }
@@ -466,11 +460,6 @@ inline bool v4_ok(const void* a, const void* b, const void* c, const void* d, co
   return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
            reinterpret_cast<uintptr_t>(d) | reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(f)) & 15) == 0;
 }
-inline int ew_grid(cgan_ctx* ctx, long long n) {
-  long long b = (n + 255) / 256;
-  long long cap = (long long)ctx->num_sms * 16;
-  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
-}
 
 }  // namespace
 
@@ -582,8 +571,6 @@ static int gemv_rows(cgan_ctx* ctx, float* out, const float* w, const float* b, 
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }
-
-int cgan_scale_by_dev(cgan_ctx*, float*, const float*, const float*, float, int, int64_t);
 
 int cgan_spectral_norm(cgan_ctx* ctx, const float* w, int rows, int cols, int left, float eps, float* u, float* v,
                        float* sigma, float* wbar) {

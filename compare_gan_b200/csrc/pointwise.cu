@@ -105,12 +105,6 @@ int64_t cgan_launch_count(cgan_ctx* ctx) { return ctx ? ctx->launches : -1; }
 
 namespace {
 
-inline int ew_grid(cgan_ctx* ctx, long long n) {
-  long long b = (n + 255) / 256;
-  long long cap = (long long)ctx->num_sms * 16;
-  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
-}
-
 #define EW_LOOP(i, n)                                                                  \
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x, s__ = (long long)gridDim.x * blockDim.x; \
        i < (n); i += s__)
@@ -180,11 +174,6 @@ __global__ void bias_add_kernel(float* __restrict__ y, const float* __restrict__
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-__device__ __forceinline__ float rna_tf32_(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
 __device__ __forceinline__ float act_fwd_1(float v, int kind, float leak) {
   if (kind == CGAN_ACT_RELU) return fmaxf(v, 0.f);
   if (kind == CGAN_ACT_LRELU) return fmaxf(v, leak * v);
@@ -206,12 +195,12 @@ __global__ void act_fwd_kernel(float* __restrict__ y, const float* __restrict__ 
   EW_LOOP(i, n4) {
     float4 v = x4[i];
     v.x = act_fwd_1(v.x, kind, leak); v.y = act_fwd_1(v.y, kind, leak); v.z = act_fwd_1(v.z, kind, leak); v.w = act_fwd_1(v.w, kind, leak);
-    if (rnd) { v.x = rna_tf32_(v.x); v.y = rna_tf32_(v.y); v.z = rna_tf32_(v.z); v.w = rna_tf32_(v.w); }
+    if (rnd) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); v.z = rna_tf32(v.z); v.w = rna_tf32(v.w); }
     y4[i] = v;
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float v = act_fwd_1(x[i], kind, leak);
-    y[i] = rnd ? rna_tf32_(v) : v;
+    y[i] = rnd ? rna_tf32(v) : v;
   }
 }
 __global__ void act_bwd_kernel(float* __restrict__ dx, const float* __restrict__ dy, const float* __restrict__ ref,
@@ -225,12 +214,12 @@ __global__ void act_bwd_kernel(float* __restrict__ dx, const float* __restrict__
     float4 g = g4[i], r = r4[i];
     g.x = act_bwd_1(g.x, r.x, kind, leak); g.y = act_bwd_1(g.y, r.y, kind, leak);
     g.z = act_bwd_1(g.z, r.z, kind, leak); g.w = act_bwd_1(g.w, r.w, kind, leak);
-    if (rnd) { g.x = rna_tf32_(g.x); g.y = rna_tf32_(g.y); g.z = rna_tf32_(g.z); g.w = rna_tf32_(g.w); }
+    if (rnd) { g.x = rna_tf32(g.x); g.y = rna_tf32(g.y); g.z = rna_tf32(g.z); g.w = rna_tf32(g.w); }
     o4[i] = g;
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float g = act_bwd_1(dy[i], ref[i], kind, leak);
-    dx[i] = rnd ? rna_tf32_(g) : g;
+    dx[i] = rnd ? rna_tf32(g) : g;
   }
 }
 // generic tail of the fused convolution entry points on the exact-fp32 paths: y = round(mask(relu(y + residual)))
@@ -244,7 +233,7 @@ __global__ void conv_post_kernel(float* __restrict__ y, long long rows, int c, i
     if (residual) v += residual[o];
     if (relu) v = fmaxf(v, 0.f);
     if (mask) v = mask[o] > 0.f ? v : leak * v;
-    if (round_out) v = rna_tf32_(v);
+    if (round_out) v = rna_tf32(v);
     y[o] = v;
   }
 }
@@ -341,12 +330,12 @@ __global__ void add_kernel(float* __restrict__ y, const float* __restrict__ a, c
   EW_LOOP(i, n4) {
     float4 u = a4[i], v = b4[i];
     u.x += v.x; u.y += v.y; u.z += v.z; u.w += v.w;
-    if (rnd) { u.x = rna_tf32_(u.x); u.y = rna_tf32_(u.y); u.z = rna_tf32_(u.z); u.w = rna_tf32_(u.w); }
+    if (rnd) { u.x = rna_tf32(u.x); u.y = rna_tf32(u.y); u.z = rna_tf32(u.z); u.w = rna_tf32(u.w); }
     y4[i] = u;
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float v = a[i] + b[i];
-    y[i] = rnd ? rna_tf32_(v) : v;
+    y[i] = rnd ? rna_tf32(v) : v;
   }
 }
 __global__ void avgpool2_fwd_kernel(float* __restrict__ y, const float* __restrict__ x, int n, int h, int w, int c) {

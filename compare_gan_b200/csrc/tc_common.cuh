@@ -88,13 +88,6 @@ __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-__device__ __forceinline__ float rna_tf32(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-
-
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -125,6 +118,17 @@ inline bool make_act_map(CUtensorMap* tm, const float* base, int c, int w, int h
   return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, es,
              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// map of view v of an operand (views past a.nviews repeat view 0)
+inline bool make_view_map(CUtensorMap* tm, const TcView& a, int v, int bw, int bh, int bni,
+                          CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+  int vv = v < a.nviews ? v : 0;
+  // stride-2 phase views of an odd-sized tensor differ in extent: rows 2r+a < H  =>  (H - a + 1) / 2 rows in phase a
+  int vh = a.h, vw = a.w;
+  if (a.nviews == 4 && a.phase_h > 0) { vh = (a.phase_h - (vv >> 1) + 1) / 2; vw = (a.phase_w - (vv & 1) + 1) / 2; }
+  if (vh < 1 || vw < 1) { vh = a.h; vw = a.w; vv = 0; }
+  return make_act_map(tm, a.in + a.view_off[vv], a.ch, vw, vh, a.n, a.sw, a.sh, a.sn, bw, bh, bni, swizzle);
 }
 
 }  // namespace tc

@@ -254,11 +254,7 @@ fwd_thin3_kernel(const float* __restrict__ x, const float* __restrict__ w, const
 #pragma unroll
         for (int m = 0; m < M; ++m) acc = fmaf(xv[m], wr[m], acc);
         if (relu) acc = fmaxf(acc, 0.f);
-        if (round_out) {                     // the consumer is a tensor-core convolution: store TF32-representable values
-          uint32_t u;
-          asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(acc));
-          acc = __uint_as_float(u);
-        }
+        if (round_out) acc = rna_tf32(acc);  // the consumer is a tensor-core convolution: store TF32-representable values
         yrow[(size_t)pi * p.ld] = acc;
       }
     }
@@ -321,14 +317,6 @@ inline bool thin3_params(const cgan_conv_desc* d, int num_sms, int ctas_per_sm, 
   return true;
 }
 
-__global__ void thin_reduce_kernel(float* __restrict__ out, const float* __restrict__ part, long long n, int blocks) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float s = 0.f;
-  for (int b = 0; b < blocks; ++b) s += part[(long long)b * n + i];
-  out[i] = s;
-}
-
 }  // namespace
 
 // ---- 1x1 kernels over <= 4 input channels (the shortcut of BigGAN's first discriminator block, resnet_biggan.py:
@@ -336,12 +324,6 @@ __global__ void thin_reduce_kernel(float* __restrict__ out, const float* __restr
 // Both are streams over the [pixels, cout] tensor: the forward writes it once (thread = 4 output channels of one pixel,
 // filter rows in registers; residual add, ReLU and TF32 rounding fused), the filter gradient reads it once (thread =
 // output channel, PWT_U pixels in flight, one partial [cin, cout] per CTA).
-__device__ __forceinline__ float thin_rna(float v) {
-  unsigned u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-  return __uint_as_float(u);
-}
-
 template <int CIN>
 __global__ void fwd_pw_thin_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                                    float* __restrict__ y, const float* __restrict__ residual, long long npix, int cout,
@@ -364,7 +346,7 @@ __global__ void fwd_pw_thin_kernel(const float* __restrict__ x, const float* __r
       acc.x += r.x; acc.y += r.y; acc.z += r.z; acc.w += r.w;
     }
     if (relu) { acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f); }
-    if (round_out) { acc.x = thin_rna(acc.x); acc.y = thin_rna(acc.y); acc.z = thin_rna(acc.z); acc.w = thin_rna(acc.w); }
+    if (round_out) { acc.x = rna_tf32(acc.x); acc.y = rna_tf32(acc.y); acc.z = rna_tf32(acc.z); acc.w = rna_tf32(acc.w); }
     *reinterpret_cast<float4*>(y + o) = acc;
   }
 }
@@ -459,9 +441,7 @@ int cgan_wgrad_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, cons
       default: wgrad_pw_thin_kernel<4><<<grid, 128, 0, ctx->stream>>>(x, dy, partial, p.npix, d->cout, ppb); break;
     }
     CGAN_LAUNCHED(ctx);
-    thin_reduce_kernel<<<cdiv(wn, 256), 256, 0, ctx->stream>>>(dw, partial, wn, blocks);
-    CGAN_LAUNCHED(ctx);
-    return CGAN_OK;
+    return cgan_splitk_reduce(ctx, dw, partial, wn, blocks);
   }
   if (d->cin <= 4 && d->kh == 3 && d->kw == 3) {
     Thin3Params q;
@@ -481,9 +461,7 @@ int cgan_wgrad_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, cons
         default: wgrad_thin3_kernel<4><<<grid, 128, 0, ctx->stream>>>(x, dy, partial, q); break;
       }
       CGAN_LAUNCHED(ctx);
-      thin_reduce_kernel<<<cdiv(wn, 256), 256, 0, ctx->stream>>>(dw, partial, wn, blocks);
-      CGAN_LAUNCHED(ctx);
-      return CGAN_OK;
+      return cgan_splitk_reduce(ctx, dw, partial, wn, blocks);
     }
   }
   long long want_blocks = 4ll * ctx->num_sms;
@@ -510,9 +488,7 @@ int cgan_wgrad_thin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, cons
     wgrad_thin_cout_kernel<9, 3><<<grid, threads, 0, ctx->stream>>>(x, dy, partial, p);
   }
   CGAN_LAUNCHED(ctx);
-  thin_reduce_kernel<<<cdiv(wn, 256), 256, 0, ctx->stream>>>(dw, partial, wn, blocks);
-  CGAN_LAUNCHED(ctx);
-  return CGAN_OK;
+  return cgan_splitk_reduce(ctx, dw, partial, wn, blocks);
 }
 
 

@@ -19,9 +19,6 @@
 // accumulation — the same as every other tensor-core contraction of math_mode 1 (CGAN_PATH_TCGEN05_TF32).
 #include "common.cuh"
 
-bool cgan_wgrad_tc_geometry_ok(int n, int h, int w);
-int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw, int x_tf32, int dy_tf32);
-
 namespace {
 
 constexpr int TT_K = 32;                        // patch row: 32 floats = one 128-byte TMA / swizzle row
@@ -32,12 +29,6 @@ struct TapList {
   int ntaps, c, k;                              // k = ntaps * c <= 32
   int off_h[TT_MAX_TAPS], off_w[TT_MAX_TAPS];
 };
-
-__device__ __forceinline__ float tt_rna(float v) {
-  unsigned u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-  return __uint_as_float(u);
-}
 
 // out[(n, gy, gx)][m], m = tap*C + c  =  src[n, gy*stride + off_h[tap], gx*stride + off_w[tap], c]  (0 outside / m >= K).
 // One thread per (pixel, 4 consecutive m): eight threads write one 128-byte row.  A thread keeps its quarter-row index for
@@ -70,7 +61,7 @@ patch_kernel(float* __restrict__ out, const float* __restrict__ src, TapList t, 
     for (int j = 0; j < 4; ++j) {
       const int y = gy * stride + dy[j], x = gx * stride + dx[j];
       const bool ok = live[j] && y >= 0 && y < sh && x >= 0 && x < sw;
-      v[j] = ok ? tt_rna(__ldg(base + ((size_t)y * sw + x) * t.c + cc[j])) : 0.f;
+      v[j] = ok ? rna_tf32(__ldg(base + ((size_t)y * sw + x) * t.c + cc[j])) : 0.f;
     }
     *reinterpret_cast<float4*>(out + (size_t)pix * TT_K + q * 4) = make_float4(v[0], v[1], v[2], v[3]);
   }
@@ -145,14 +136,23 @@ inline void tap_list(const cgan_conv_desc* d, int sign, int c, TapList* t) {
 inline TcConv tc_gemm(const float* x, int n, int h, int w, int kdim, const float* wsrc, int transpose_w, int ncols, float* y,
                       int ldy) {
   TcConv c = {};
-  tc_in_dense(&c, x, n, h, w, kdim);
+  tc_in_dense(&c.a, x, n, h, w, kdim);
   c.wsrc = wsrc; c.taps_total = 1; c.transpose_w = transpose_w; c.ncols = ncols;
   c.taps.ntaps = 1;
   tc_out_dense(&c, y, h, w, ldy);
   return c;
 }
 
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+// dw[xch][dych] = x^T dy over dense NHWC operands on an n x h x w grid: the filter gradient of a 1x1 convolution
+inline TcWgrad tc_gemm_tn(int n, int h, int w, const float* x, int xch, int x_tf32, const float* dy, int dych, int dy_tf32,
+                          float* dw) {
+  TcWgrad g = {};
+  tc_in_dense(&g.x, x, n, h, w, xch);
+  tc_in_dense(&g.dy, dy, n, h, w, dych);
+  g.x.tf32 = x_tf32; g.dy.tf32 = dy_tf32;
+  g.taps.ntaps = 1; g.taps_total = 1; g.dw = dw;
+  return g;
+}
 
 // workspace: [0, TT_RESERVE) for the GEMM kernels' own use | patch / T tensor | small weight buffers (2 x 64 KB)
 inline int tt_workspace(cgan_ctx* ctx, long long pixels, float** big, float** small0, float** small1) {
@@ -201,8 +201,11 @@ int cgan_thin_tc_fwd_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x,
   return cgan_conv_tc(ctx, c);
 }
 
+// The filter-gradient products below read the patch tensor and write into the workspace, whose slices are 256-byte
+// aligned, and the caller checks the alignment of x and dy: their _ok tests describe them with null pointers.
 bool cgan_thin_tc_wgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
-  return cgan_thin_tc_cin_ok(ctx, d) && d->cout <= 256 && cgan_wgrad_tc_geometry_ok(d->n, d->oh, d->ow);
+  return cgan_thin_tc_cin_ok(ctx, d) && d->cout <= 256 &&
+         cgan_wgrad_tc_fits(tc_gemm_tn(d->n, d->oh, d->ow, nullptr, TT_K, 1, nullptr, d->cout, 0, nullptr));
 }
 
 int cgan_thin_tc_wgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, int dy_tf32, float* dw) {
@@ -214,10 +217,8 @@ int cgan_thin_tc_wgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   tap_list(d, 1, d->cin, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, x, t, d->n, d->oh, d->ow, d->h, d->w, d->stride);
   CGAN_LAUNCHED(ctx);
-  cgan_conv_desc g;          // dW32[32][cout] = P^T dy: the filter gradient of a 1x1 convolution 32 -> cout on the output grid
-  memset(&g, 0, sizeof(g));
-  g.n = d->n; g.h = g.oh = d->oh; g.w = g.ow = d->ow; g.cin = TT_K; g.cout = d->cout; g.kh = g.kw = 1; g.stride = 1;
-  rc = cgan_wgrad_tc(ctx, &g, pt, dy, s0, 1, dy_tf32);
+  // dW32[32][cout] = P^T dy over the output grid
+  rc = cgan_wgrad_tc(ctx, tc_gemm_tn(d->n, d->oh, d->ow, pt, TT_K, 1, dy, d->cout, dy_tf32, s0));
   if (rc) return rc;
   return cgan_copy(ctx, dw, s0, (int64_t)t.k * d->cout);          // rows [0, K) of dW32 are HWIO's [kh][kw][cin][cout]
 }
@@ -300,7 +301,8 @@ int cgan_thin_tc_dgrad_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float*
 }
 
 bool cgan_thin_tc_wgrad_cout_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
-  return cgan_thin_tc_cout_ok(ctx, d) && d->cin % 32 == 0 && d->cin >= 64 && cgan_wgrad_tc_geometry_ok(d->n, d->h, d->w) &&
+  return cgan_thin_tc_cout_ok(ctx, d) && d->cin >= 64 &&
+         cgan_wgrad_tc_fits(tc_gemm_tn(d->n, d->h, d->w, nullptr, d->cin, 0, nullptr, TT_K, 1, nullptr)) &&
          (size_t)2 * ctx->num_sms * TT_K * d->cin * 4 <= TT_RESERVE && (size_t)d->cin * TT_K * 4 <= (64u << 10);
 }
 
@@ -313,10 +315,8 @@ int cgan_thin_tc_wgrad_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float*
   tap_list(d, -1, d->cout, &t);
   patch_kernel<<<ew_blocks(ctx, pixels * 8), 256, 0, ctx->stream>>>(pt, dy, t, d->n, d->h, d->w, d->oh, d->ow, 1);
   CGAN_LAUNCHED(ctx);
-  cgan_conv_desc g;          // dW'[cin][32] = x^T P
-  memset(&g, 0, sizeof(g));
-  g.n = d->n; g.h = g.oh = d->h; g.w = g.ow = d->w; g.cin = d->cin; g.cout = TT_K; g.kh = g.kw = 1; g.stride = 1;
-  rc = cgan_wgrad_tc(ctx, &g, x, pt, dwp, x_tf32, 1);
+  // dW'[cin][32] = x^T P
+  rc = cgan_wgrad_tc(ctx, tc_gemm_tn(d->n, d->h, d->w, x, d->cin, x_tf32, pt, TT_K, 1, dwp));
   if (rc) return rc;
   hwio_from_wcols_kernel<<<cdiv((long long)t.k * d->cin, 256), 256, 0, ctx->stream>>>(dw, dwp, t.ntaps, d->cin, d->cout, TT_K);
   CGAN_LAUNCHED(ctx);

@@ -213,15 +213,9 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   }
 }
 
-__global__ void wg_reduce_kernel(float* __restrict__ out, const float* __restrict__ part, long long n, int splits) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float s = 0.f;
-  for (int z = 0; z < splits; ++z) s += part[(long long)z * n + i];
-  out[i] = s;
-}
-
+// the n x h x w pixel grid cut into 32-pixel TMA boxes of bw x bh x bni
 bool box32(int n, int h, int w, int* bw, int* bh, int* bni) {
+  if (n < 1 || h < 1 || w < 1) return false;
   int b = w < 32 ? w : 32;
   if (32 % b != 0 || w % b != 0) return false;
   int hh = 32 / b; if (hh > h) hh = h;
@@ -277,152 +271,82 @@ int wg_launch(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BM
 
 }  // namespace
 
-// can the pixel loop of a stride-1 n x h x w grid be cut into 32-pixel TMA boxes?
-bool cgan_wgrad_tc_geometry_ok(int n, int h, int w) {
+bool cgan_wgrad_tc_fits(const TcWgrad& g) {
   int bw, bh, bni;
-  return box32(n, h, w, &bw, &bh, &bni);
+  return box32(g.dy.n, g.dy.h, g.dy.w, &bw, &bh, &bni) && (!g.per_image || (bni == 1 && g.dy.n <= 65535)) &&
+         g.x.ch > 0 && g.x.ch % 32 == 0 &&            // ci tiles of 128, the last one zero-padded
+         pick_bn(g.dy.ch) != 0 && g.taps.ntaps >= 1 && g.taps.ntaps <= WG_MAX_TAPS && al16(g.x.in) && al16(g.dy.in) &&
+         al16(g.dw);
 }
 
-bool cgan_wgrad_tc_ok(const cgan_conv_desc* d) {
-  if ((d->stride != 1 && d->stride != 2) || d->kh * d->kw > WG_MAX_TAPS) return false;
-  if (d->stride == 2) {
-    if (d->upsample || (d->h & 1) || (d->w & 1) || d->oh != d->h / 2 || d->ow != d->w / 2) return false;
-    if (d->cin % 32 != 0 || d->cin < 64 || pick_bn(d->cout) == 0) return false;
-    int bw, bh, bni;
-    return box32(d->n, d->oh, d->ow, &bw, &bh, &bni);
-  }
-  if (d->cin % 32 != 0 || d->cin < 64 || pick_bn(d->cout) == 0) return false;   // Cin tiles of 128, last one zero-padded
-  if (d->oh != (d->upsample ? 2 * d->h : d->h) || d->ow != (d->upsample ? 2 * d->w : d->w)) return false;
-  int bw, bh, bni;
-  return box32(d->n, d->h, d->w, &bw, &bh, &bni);
-}
-
-int cgan_wgrad_tc(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x, const float* dy, float* dw, int x_tf32, int dy_tf32) {
+int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
+  if (!cgan_wgrad_tc_fits(g)) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: shape%s", "cgan_wgrad_tc");
   WgParams p;
   memset(&p, 0, sizeof(p));
-  p.round_a = x_tf32 ? 0 : 1;
-  p.round_b = dy_tf32 ? 0 : 1;
-  const int gh = d->stride == 2 ? d->oh : d->h, gw = d->stride == 2 ? d->ow : d->w;     // pixel-loop grid
-  if (!box32(d->n, gh, gw, &p.bw, &p.bh, &p.bni)) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: geometry%s", "cgan_wgrad_tc");
+  const int n = g.dy.n, gh = g.dy.h, gw = g.dy.w;      // the pixel grid
+  p.round_a = g.x.tf32 ? 0 : 1;
+  p.round_b = g.dy.tf32 ? 0 : 1;
+  box32(n, gh, gw, &p.bw, &p.bh, &p.bni);
   p.tiles_w = gw / p.bw;
   p.tiles_h = gh / p.bh;
-  p.kblocks = (int)((long long)d->n * gh * gw / WG_P);
-  p.bn = pick_bn(d->cout);
-  p.ci_tiles = (d->cin + 127) / 128;
-  p.co_tiles = (d->cout + p.bn - 1) / p.bn;
-  p.cin = d->cin; p.cout = d->cout; p.taps_total = d->kh * d->kw;
-  // taps: the pixel loop runs over a grid (i, j) of gh x gw cells: the input grid (stride 1, incl. zero-inserted
-  // inputs) or the output grid (stride 2); tap (kh,kw) pairs X view `amap` at [i+dh, j+dw] with dY view `bmap` at [i, j].
-  // Stride 2: output (i,j) reads input row 2i + kh - pad_t = 2(i + dh) + a, phase view a of X.  Zero-inserted input:
-  // output row 2i+a reads virtual row 2i+a+kh-pad_t, real only when even, from dY phase view a = (pad_t - kh) & 1.
-  ConvTaps t;
-  conv_taps(d, d->upsample ? -1 : 1, d->stride == 2 ? TAP_VIEW : d->upsample ? TAP_PHASE : TAP_DIRECT, &t);
-  const int nt = t.ntaps;
-  for (int i = 0; i < nt; ++i) {
+  p.kblocks = (int)((long long)n * gh * gw / WG_P);
+  p.bn = pick_bn(g.dy.ch);
+  p.ci_tiles = (g.x.ch + 127) / 128;
+  p.co_tiles = (g.dy.ch + p.bn - 1) / p.bn;
+  p.cin = g.x.ch; p.cout = g.dy.ch; p.taps_total = g.taps_total;
+  // tap i pairs x view amap[i] at [y + off_h, x + off_w] with dy view bmap[i] at [y, x]
+  const ConvTaps& t = g.taps;
+  p.ntaps = t.ntaps;
+  for (int i = 0; i < t.ntaps; ++i) {
     p.off_h[i] = t.off_h[i]; p.off_w[i] = t.off_w[i]; p.wtap[i] = t.wtap[i];
-    p.amap[i] = d->upsample ? 0 : t.view[i];
-    p.bmap[i] = d->upsample ? t.view[i] : 0;
+    p.amap[i] = g.taps_view_dy ? 0 : t.view[i];
+    p.bmap[i] = g.taps_view_dy ? t.view[i] : 0;
   }
-  p.ntaps = nt;
   // two (tap, ci-tile) units per CTA when they read the same dY view: dY is then fetched once per k-block for both
-  const int units = p.ci_tiles * nt;
+  const int units = p.ci_tiles * t.ntaps;
   bool same_b = true;
-  for (int i = 1; i < nt; ++i) same_b = same_b && p.bmap[i] == p.bmap[0];
-  p.mt = (ctx->tc_mt_max >= 2 && same_b && units >= 2 && 2 * p.bn <= WG_ACC_COLS) ? 2 : 1;
+  for (int i = 1; i < t.ntaps; ++i) same_b = same_b && p.bmap[i] == p.bmap[0];
+  p.mt = (!g.per_image && ctx->tc_mt_max >= 2 && same_b && units >= 2 && 2 * p.bn <= WG_ACC_COLS) ? 2 : 1;
   const size_t stage_bytes = (size_t)p.mt * WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
-  const bool two_ctas = wg_smem(stage_bytes, 110 * 1024, &p.stages) <= 113 * 1024;
-  long long tiles = (long long)p.co_tiles * ((units + p.mt - 1) / p.mt);
-  // two CTAs per SM in total (two waves when only one fits), rounded DOWN so the grid never spills a few CTAs into an
-  // extra wave; the pixel chain each fp32 accumulator sums stays as short as with two resident CTAs per SM
-  int splits = (int)((2ll * ctx->num_sms) / tiles);
-  int max_splits = p.kblocks / 8 > 0 ? p.kblocks / 8 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  p.kb_per_split = (p.kblocks + splits - 1) / splits;
-  splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
+  const long long tiles = (long long)p.co_tiles * ((units + p.mt - 1) / p.mt);
+  int splits;
+  size_t smem;
+  if (g.per_image) {
+    // "split" i = image i: its partial tile IS the result dw[i]
+    p.kb_per_split = gh * gw / WG_P;
+    splits = n;
+    smem = wg_smem(stage_bytes, 110 * 1024, &p.stages);
+  } else {
+    const bool two_ctas = wg_smem(stage_bytes, 110 * 1024, &p.stages) <= 113 * 1024;
+    // two CTAs per SM in total (two waves when only one fits), rounded DOWN so the grid never spills a few CTAs into an
+    // extra wave; the pixel chain each fp32 accumulator sums stays as short as with two resident CTAs per SM
+    splits = (int)((2ll * ctx->num_sms) / tiles);
+    int max_splits = p.kblocks / 8 > 0 ? p.kblocks / 8 : 1;
+    if (splits > max_splits) splits = max_splits;
+    if (splits < 1) splits = 1;
+    p.kb_per_split = (p.kblocks + splits - 1) / splits;
+    splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
+    smem = wg_smem(stage_bytes, two_ctas ? 110 * 1024 : 220 * 1024, &p.stages);
+  }
 
-  long long wn = (long long)p.taps_total * d->cin * d->cout;
-  float* partial = dw;
-  if (splits > 1) {
+  const bool reduce = !g.per_image && splits > 1;
+  const long long wn = (long long)p.taps_total * p.cin * p.cout;
+  p.partial = g.dw;
+  if (reduce) {
     void* ws = nullptr;
     int rc = cgan_ws(ctx, (size_t)splits * wn * sizeof(float), &ws);
     if (rc) return rc;
-    partial = reinterpret_cast<float*>(ws);
+    p.partial = reinterpret_cast<float*>(ws);
   }
-  p.partial = partial;
 
   BMaps tm_x, tm_dy;
   memset(&tm_x, 0, sizeof(tm_x));
   memset(&tm_dy, 0, sizeof(tm_dy));
-  for (int v = 0; v < 4; ++v) {
-    bool ok;
-    if (d->stride == 2) {     // X seen through its four stride-2 phases, each of the OUTPUT's spatial size
-      int a = v >> 1, b = v & 1;
-      ok = make_act_map(&tm_x.m[v], x + ((long long)a * d->w + b) * d->cin, d->cin, gw, gh, d->n, 2ll * d->cin,
-                        2ll * d->w * d->cin, (long long)d->h * d->w * d->cin, p.bw, p.bh, p.bni,
-                        CU_TENSOR_MAP_SWIZZLE_NONE);
-    } else {
-      ok = make_act_map(&tm_x.m[v], x, d->cin, d->w, d->h, d->n, d->cin, (long long)d->w * d->cin,
-                        (long long)d->h * d->w * d->cin, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE);
-    }
-    if (!ok) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(x) failed%s", "cgan_wgrad_tc");
-  }
-  for (int v = 0; v < 4; ++v) {
-    bool ok;
-    if (!d->upsample) {
-      ok = make_act_map(&tm_dy.m[v], dy, d->cout, gw, gh, d->n, d->cout, (long long)d->ow * d->cout,
-                        (long long)d->oh * d->ow * d->cout, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE);
-    } else {
-      int a = v >> 1, b = v & 1;
-      ok = make_act_map(&tm_dy.m[v], dy + ((long long)a * d->ow + b) * d->cout, d->cout, d->w, d->h, d->n, 2ll * d->cout,
-                        2ll * d->ow * d->cout, (long long)d->oh * d->ow * d->cout, p.bw, p.bh, p.bni,
-                        CU_TENSOR_MAP_SWIZZLE_NONE);
-    }
-    if (!ok) return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(dy) failed%s", "cgan_wgrad_tc");
-  }
-  const size_t smem = wg_smem(stage_bytes, two_ctas ? 110 * 1024 : 220 * 1024, &p.stages);
+  for (int v = 0; v < 4; ++v)
+    if (!make_view_map(&tm_x.m[v], g.x, v, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE) ||
+        !make_view_map(&tm_dy.m[v], g.dy, v, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE))
+      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed%s", "cgan_wgrad_tc");
   int rc = wg_launch(ctx, dim3((unsigned)tiles, (unsigned)splits), smem, tm_x, tm_dy, p);
-  if (rc) return rc;
-  if (splits > 1) {
-    wg_reduce_kernel<<<cdiv(wn, 256), 256, 0, ctx->stream>>>(dw, partial, wn, splits);
-    CGAN_LAUNCHED(ctx);
-  }
-  return CGAN_OK;
-}
-
-
-// C[i][k1, k2] = sum_pixels A[i][pixel, k1] * B[i][pixel, k2]   (per-image A^T B; attention's d(phi), d(g))
-int cgan_wgrad_tc_batched(cgan_ctx* ctx, const float* a, const float* b, float* c, int batch, int h, int w, int k1, int k2) {
-  WgParams p;
-  memset(&p, 0, sizeof(p));
-  if (!box32(1, h, w, &p.bw, &p.bh, &p.bni) || p.bni != 1)
-    return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: geometry%s", "cgan_wgrad_tc_batched");
-  p.tiles_w = w / p.bw;
-  p.tiles_h = h / p.bh;
-  const int kb_per_image = h * w / WG_P;
-  p.kblocks = kb_per_image * batch;
-  p.kb_per_split = kb_per_image;            // "split" i = image i: its partial tile IS the result C[i]
-  p.bn = pick_bn(k2);
-  if (p.bn == 0) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: columns%s", "cgan_wgrad_tc_batched");
-  p.ci_tiles = (k1 + 127) / 128;
-  p.co_tiles = (k2 + p.bn - 1) / p.bn;
-  p.cin = k1; p.cout = k2; p.taps_total = 1;
-  p.ntaps = 1;
-  p.mt = 1;
-  p.round_a = p.round_b = 1;
-  p.partial = c;
-  BMaps tm_x, tm_dy;
-  memset(&tm_x, 0, sizeof(tm_x));
-  memset(&tm_dy, 0, sizeof(tm_dy));
-  for (int v = 0; v < 4; ++v) {
-    if (!make_act_map(&tm_x.m[v], a, k1, w, h, batch, k1, (long long)w * k1, (long long)h * w * k1, p.bw, p.bh, p.bni,
-                      CU_TENSOR_MAP_SWIZZLE_NONE) ||
-        !make_act_map(&tm_dy.m[v], b, k2, w, h, batch, k2, (long long)w * k2, (long long)h * w * k2, p.bw, p.bh, p.bni,
-                      CU_TENSOR_MAP_SWIZZLE_NONE))
-      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed%s", "cgan_wgrad_tc_batched");
-  }
-  const size_t stage_bytes = WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
-  const size_t smem = wg_smem(stage_bytes, 110 * 1024, &p.stages);
-  if (batch > 65535) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: batch exceeds grid.y%s", "cgan_wgrad_tc_batched");
-  return wg_launch(ctx, dim3((unsigned)(p.ci_tiles * p.co_tiles), (unsigned)batch), smem, tm_x, tm_dy, p);
+  if (rc || !reduce) return rc;
+  return cgan_splitk_reduce(ctx, g.dw, p.partial, wn, splits);
 }
