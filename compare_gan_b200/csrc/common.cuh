@@ -19,6 +19,7 @@ struct cgan_ctx {
   int tc_halo;         // 3x3 stride-1 tensor-core convolutions use the halo variant (CGAN_OPT_TC_HALO / env CGAN_TC_HALO, default 1)
   int tc_thin;         // image-side (<= 4 channel) convolutions through 32-wide patch tensors on wgmma (CGAN_OPT_TC_THIN / env CGAN_TC_THIN)
   int last_path;       // CGAN_PATH_* of the most recent contraction (cgan_ctx_get_option(CGAN_OPT_LAST_PATH))
+  int last_tc_bn, last_tc_mt, last_tc_halo;   // geometry of the most recent conv_tc launch (CGAN_OPT_LAST_TC_*)
   unsigned* counters;  // CGAN_NUM_COUNTERS zero-initialised tickets for single-launch two-stage reductions (norm.cu)
   void* p2p;           // peer-memory all-reduce state (p2p.cu), null until cgan_p2p_local_handle
   char err[512];

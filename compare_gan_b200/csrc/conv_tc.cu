@@ -491,6 +491,7 @@ int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& a
 
 // the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS
 int tc_launch(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
+  ctx->last_tc_bn = p.bn; ctx->last_tc_mt = p.mt; ctx->last_tc_halo = halo ? 1 : 0;
 #define TC_CASE(BN, MT) \
   if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p);
   TC_CASE(32, 1) TC_CASE(64, 1) TC_CASE(96, 1) TC_CASE(128, 1) TC_CASE(160, 1) TC_CASE(192, 1) TC_CASE(224, 1)
