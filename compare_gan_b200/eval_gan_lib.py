@@ -1,6 +1,7 @@
 """Evaluation of a trained GAN (reference eval_gan_lib.py:65-212): sample the generator in inference mode in batches
-of 64, run Inception on the samples, compute FID / IS / KID.  Everything up to the [N,2048] statistics stays on the
-GPU; sample generation can be sharded across ranks with a final all-reduce of the statistics."""
+of 64, run Inception on the samples, compute FID / IS / KID (and MS-SSIM on the first generated samples when a task asks
+for images).  Everything up to the [N,2048] statistics stays on the GPU; sample generation can be sharded across ranks
+with a final all-reduce of the statistics."""
 import time
 
 import numpy as np
@@ -77,9 +78,10 @@ class _EvalBatchGraph(object):
   bit-identical features while the 17x17 and 8x8 Inception stages get `fuse` times as many pixel tiles per launch (at 64
   images they expose 145 / 32 tiles to 132 SMs).  The z / label stream is still drawn batch by batch in the same order."""
 
-  def __init__(self, gan, batch_size, acc, fuse=1):
+  def __init__(self, gan, batch_size, acc, fuse=1, keep_images=False):
     dev = K._RT["device"]
     self.ref_b, self.fuse = batch_size, fuse
+    self.keep_images, self.images = keep_images, None
     batch_size = batch_size * fuse
     self.gan, self.b, self.acc = gan, batch_size, acc
     self.z = tape.DT(torch.zeros(batch_size, gan._z_dim, device=dev))
@@ -110,12 +112,16 @@ class _EvalBatchGraph(object):
     y = K.one_hot(self.labels, g._dataset.num_classes) if g.conditional else None
     with V.use(g.store), tape.no_record():
       imgs = g.generator(self.z, y=y, is_training=False)
+    if self.keep_images:      # G's output in a persistent buffer (allocated by the warm-up, before capture)
+      if self.images is None:
+        self.images = K.empty(*imgs.shape)
+      K.copy_(self.images, imgs)
     pool, logits = eval_utils.inception_transform(imgs)
     K._call("cov_accumulate", pool.ptr, self.b, self.acc.dim, self.acc.s.data_ptr(), self.acc.sxx.data_ptr())
     K.copy_(self.pool, pool)
     K.copy_(self.logits, logits)
 
-  def run_batches(self, rng, num_batches):
+  def run_batches(self, rng, num_batches, keeper):
     """Draws the latents of all batches first (same RNG order as the eager path: z then labels, batch by batch), ships
     them to the device in one copy, then replays the graph back to back with no host synchronisation in between."""
     g = self.gan
@@ -138,9 +144,30 @@ class _EvalBatchGraph(object):
         self.labels.t.copy_(l_all[i], non_blocking=True)
       self.graph.replay()
       self.acc.n += self.b
+      if self.images is not None:
+        keeper.add(self.images)
       if self.acc.keep:     # device-side copies; one device->host transfer at finish()
         self.acc.acts.append(self.pool.t.clone())
         self.acc.logits.append(self.logits.t.clone())
+
+
+class _ImageKeeper(object):
+  """The first `n` generated images of one averaging run, kept on the device for the tasks that read images (MS-SSIM)."""
+
+  def __init__(self, n):
+    self.n, self.parts, self.have = n, [], 0
+
+  def add(self, imgs, valid=None):
+    take = min(self.n - self.have, imgs.shape[0] if valid is None else valid)
+    if take > 0:
+      self.parts.append(imgs.t[:take].clone())
+      self.have += take
+
+  def images255(self):
+    if not self.parts:
+      return None
+    with tape.no_record():
+      return K.affine(tape.DT(torch.cat(self.parts)), 255.0)
 
 
 def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size=64, seed=42, num_accu_examples=204800,
@@ -154,28 +181,31 @@ def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size
   rng = np.random.RandomState(seed + 1000 * rank)
   K.sync_stream()
   fake_dsets, timings = [], []
+  n_images = max([getattr(task, "images_needed", 0) for task in eval_tasks] + [0])
   with use_ema_weights(gan):
     _update_bn_accumulators(gan, batch_size, num_accu_examples, rng)
     for _ in range(num_averaging_runs):
       acc = eval_utils.FeatureAccumulator(keep_features=keep_features)
+      keeper = _ImageKeeper(n_images)
       fuse = max(1, min(int(fuse_batches), n_local // (4 * batch_size)))
-      graph = _EvalBatchGraph(gan, batch_size, acc, fuse) if (use_graph and n_local >= 4 * batch_size) else None
+      graph = _EvalBatchGraph(gan, batch_size, acc, fuse, n_images > 0) if (use_graph and n_local >= 4 * batch_size) else None
       torch.cuda.synchronize()
       t0 = time.time()
       done = 0
       if graph is not None:
         nb = n_local // (batch_size * fuse)
-        graph.run_batches(rng, nb)
+        graph.run_batches(rng, nb, keeper)
         done += nb * batch_size * fuse
       while done < n_local:
         imgs = generate_batch(gan, batch_size, rng)
         pool, logits = eval_utils.inception_transform(imgs)
         valid = min(batch_size, n_local - done)
         acc.add(pool, logits, valid)
+        keeper.add(imgs, valid)
         done += valid
       torch.cuda.synchronize()
       timings.append(time.time() - t0)
-      sample = acc.finish(eval_utils.EvalDataSample())
+      sample = acc.finish(eval_utils.EvalDataSample(keeper.images255()))
       if sample.activations is not None and not np.isfinite(sample.activations).all():
         raise eval_utils.NanFoundError("NaN in generated samples")
       fake_dsets.append(sample)

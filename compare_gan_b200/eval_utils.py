@@ -15,7 +15,8 @@ class NanFoundError(Exception):
 
 class EvalDataSample(object):
   """Container for a (fake or real) evaluation set (reference eval_utils.py:56-84), extended with the streaming
-  FID moments accumulated on the device."""
+  FID moments accumulated on the device.  For a generated set `images` holds the first N samples (N = the largest
+  images_needed of the evaluation's tasks, in [0, 255], on the device), not the whole set; None when no task needs them."""
 
   def __init__(self, images=None):
     self._images = images

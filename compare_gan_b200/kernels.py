@@ -746,6 +746,19 @@ def resize_bilinear(x, oh, ow, inception_scale=False):
   return y
 
 
+def ssim_terms(images, pairs, levels, filter_size, filter_width, max_val):
+  """Per-scale SSIM terms of image pairs of one set (metrics/image_similarity.py:85-211, 239-333): images [n,h,w,c] DT
+  with values in [0, max_val], pairs int [npairs, 2] (host) indices into it.  Returns numpy [npairs, levels, c] float32:
+  the pixel mean of cs at levels 0..levels-2 and of luminance*cs at the last level, before the relu."""
+  import numpy as np
+  n, h, w, c = images.shape
+  pr = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+  out = empty(pr.shape[0], int(levels), c)
+  _call("ssim_terms", out.ptr, images.ptr, n, h, w, c, pr.ctypes.data, pr.shape[0], int(levels), int(filter_size),
+        float(filter_width), float(max_val))
+  return out.cpu()
+
+
 def globalpool(x, mean):
   """tf.reduce_mean / reduce_sum over axes [1,2] (resnet_cifar.py:156, resnet_biggan.py:405)."""
   n, h, w, c = x.shape

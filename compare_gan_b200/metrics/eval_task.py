@@ -6,6 +6,9 @@ class EvalTask(object):
   """Tasks that compute a score from generated and real Inception statistics."""
   __metaclass__ = abc.ABCMeta
   _LABEL = None
+  # how many generated images (the first ones of each averaging run, x255, on the device) the task reads from
+  # fake_dset.images; 0: none, and the evaluation keeps no images
+  images_needed = 0
 
   def metric_list(self):
     return frozenset(self._LABEL)

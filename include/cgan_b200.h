@@ -289,6 +289,18 @@ int cgan_cov_accumulate(cgan_ctx*, const float* act, int n, int d, double* sum, 
  * when `inception_scale` (eval_utils.py:157-175). */
 int cgan_resize_bilinear(cgan_ctx*, float* y, const float* x, int n, int h, int w, int c, int oh, int ow, int inception_scale);
 
+/* ---- MS-SSIM terms (metrics/image_similarity.py:85-211, 239-333) ---- */
+/* Per-scale SSIM terms of image pairs of ONE image set.  images [n,h,w,c] fp32 NHWC, values in [0, max_val];
+ * host_pairs [npairs,2] int32 HOST indices into the set (they travel to the device in the kernel parameters, so the call
+ * stays asynchronous and capturable); out [npairs, levels, c] fp32: the mean over output pixels of cs for levels
+ * 0..levels-2 and of luminance*cs for the last level, before the relu.  Level l is level l-1 average-pooled 2x2 after
+ * repeating its last row / column where a side is odd; its window is the Gaussian of width filter_width and size
+ * min(filter_size, level height, level width) (<= 64), applied VALID.  Requires h, w >= 2^(levels-1), levels <= 16.
+ * A pair's bits do not depend on the other pairs of the call; (i, j) and (j, i) give the same bits; identical images
+ * give exactly 1.  The host finishes MS-SSIM (relu, power factors, product over levels, mean over channels). */
+int cgan_ssim_terms(cgan_ctx*, float* out, const float* images, int n, int h, int w, int c, const int32_t* host_pairs,
+                    int npairs, int levels, int filter_size, float filter_width, float max_val);
+
 /* ---- cross-replica exchange of small vectors (tpu/tpu_ops.py:75-125: cross_replica_mean / cross_replica_moments) ---- */
 /* One process per GPU on one node.  Every rank allocates a communication buffer and publishes its cudaIpc handle
  * (cgan_p2p_local_handle -> 64 bytes), the host code all-gathers the handles (torch.distributed) and hands all of them
