@@ -32,7 +32,7 @@ OPT_LAST_TC_BN, OPT_LAST_TC_MT, OPT_LAST_TC_HALO = 7, 8, 9
 PATH_NAMES = {0: "simt_fp32", 1: "tcgen05_tf32", 2: "thin_fp32"}
 
 _SCALARS = {"int": ctypes.c_int, "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64,
-            "float": ctypes.c_float, "size_t": ctypes.c_size_t, "uint64_t": ctypes.c_uint64}
+            "float": ctypes.c_float, "double": ctypes.c_double, "size_t": ctypes.c_size_t, "uint64_t": ctypes.c_uint64}
 
 
 def parse_header(path=HEADER):

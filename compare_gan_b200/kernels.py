@@ -759,6 +759,40 @@ def ssim_terms(images, pairs, levels, filter_size, filter_width, max_val):
   return out.cpu()
 
 
+def kmeans_seed(x, uniforms):
+  """k-means++ centroids of `groups` independent seedings (metrics/prd_score.py:111-113): x [m, d] float32 torch tensor
+  on the device, uniforms [groups, k] float64 host values in [0, 1).  Returns [groups, k, d] float64 on the device."""
+  import numpy as np
+  m, d = x.shape
+  u = np.ascontiguousarray(uniforms, np.float64)
+  groups, k = u.shape
+  c = torch.empty(groups, k, d, dtype=torch.float64, device=_RT["device"])
+  _call("kmeans_seed", c.data_ptr(), x.data_ptr(), m, d, k, groups, u.ctypes.data)
+  return c
+
+
+def kmeans_lloyd_step(x, centroids, labels, state, tol):
+  """One Lloyd iteration of every running group, in place: centroids [groups, k, d] float64, labels [groups, m] int32,
+  state [groups, 2] int32 (status, iterations; zero before the first step)."""
+  groups, k, d = centroids.shape
+  _call("kmeans_lloyd_step", centroids.data_ptr(), labels.data_ptr(), state.data_ptr(), x.data_ptr(), x.shape[0], d, k,
+        groups, float(tol))
+
+
+def kmeans_finish(x, centroids, n_eval):
+  """Final assignment: (labels [groups, m] int32 on the device, inertia [groups] and counts [groups, 2, k] as numpy;
+  counts split at row n_eval)."""
+  groups, k, d = centroids.shape
+  m = x.shape[0]
+  dev = _RT["device"]
+  labels = torch.empty(groups, m, dtype=torch.int32, device=dev)
+  inertia = torch.empty(groups, dtype=torch.float64, device=dev)
+  counts = torch.empty(groups, 2, k, dtype=torch.int32, device=dev)
+  _call("kmeans_finish", labels.data_ptr(), inertia.data_ptr(), counts.data_ptr(), centroids.data_ptr(), x.data_ptr(), m,
+        d, k, groups, int(n_eval))
+  return labels, inertia.cpu().numpy(), counts.cpu().numpy()
+
+
 def globalpool(x, mean):
   """tf.reduce_mean / reduce_sum over axes [1,2] (resnet_cifar.py:156, resnet_biggan.py:405)."""
   n, h, w, c = x.shape

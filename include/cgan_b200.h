@@ -301,6 +301,32 @@ int cgan_resize_bilinear(cgan_ctx*, float* y, const float* x, int n, int h, int 
 int cgan_ssim_terms(cgan_ctx*, float* out, const float* images, int n, int h, int w, int c, const int32_t* host_pairs,
                     int npairs, int levels, int filter_size, float filter_width, float max_val);
 
+/* ---- k-means of the PRD histograms (metrics/prd_score.py:94-122, the MiniBatchKMeans fit of _cluster_into_bins) ---- */
+/* `groups` independent clusterings of the same points x [m,d] fp32 into k clusters (1 <= k <= 64, m >= k), in float64
+ * throughout: squared distances ||x||^2 + ||c||^2 - 2 x.c with x.c on the FP64 tensor cores (DMMA), the nearest centre
+ * being the first minimum.  Centroids are [groups, k, d] float64.  A group's results do not depend on the other groups of
+ * the call, and reruns are bit-identical.
+ *
+ * k-means++ seeding: host_uniforms [groups, k] float64 HOST values in [0, 1) (checked on the host, then copied to the
+ * workspace).  Centre 0 of group g is point min(floor(u[g,0] m), m-1); centre j is the smallest i with
+ * cumsum(w)[i] > u[g,j] * cumsum(w)[m-1], cumsum a sequential float64 sum and w[i] = max(0, squared distance of point i
+ * to its nearest chosen centre); when cumsum(w)[m-1] == 0, point min(floor(u m), m-1). */
+int cgan_kmeans_seed(cgan_ctx*, double* centroids, const float* x, int m, int d, int k, int groups,
+                     const double* host_uniforms);
+/* One Lloyd iteration (sklearn KMeans(algorithm="lloyd")) of every group whose state[g,0] is 0: assign every point to
+ * its nearest centre (labels [groups, m] int32), then move each centre to the float64 mean of its points (summed in
+ * point order; an EMPTY cluster keeps its centre).  state [groups, 2] int32, zero before the first step:
+ * (status, iterations done); status becomes 2 when the labels equal those of the group's previous step, else 1 when the
+ * total squared centre shift is <= tol, and stays 0 otherwise.  Finished groups cost nothing.  The caller reads state
+ * back to decide whether to step again (max_iter is the caller's). */
+int cgan_kmeans_lloyd_step(cgan_ctx*, double* centroids, int32_t* labels, int32_t* state, const float* x, int m, int d,
+                           int k, int groups, double tol);
+/* Final assignment against the given centroids: labels [groups, m] int32, inertia [groups] float64 (the sum of the
+ * squared distances in a fixed order), counts [groups, 2, k] int32: the points of each cluster among rows [0, n_eval)
+ * and among rows [n_eval, m). */
+int cgan_kmeans_finish(cgan_ctx*, int32_t* labels, double* inertia, int32_t* counts, const double* centroids,
+                       const float* x, int m, int d, int k, int groups, int n_eval);
+
 /* ---- cross-replica exchange of small vectors (tpu/tpu_ops.py:75-125: cross_replica_mean / cross_replica_moments) ---- */
 /* One process per GPU on one node.  Every rank allocates a communication buffer and publishes its cudaIpc handle
  * (cgan_p2p_local_handle -> 64 bytes), the host code all-gathers the handles (torch.distributed) and hands all of them
