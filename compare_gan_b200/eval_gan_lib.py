@@ -1,6 +1,6 @@
 """Evaluation of a trained GAN (reference eval_gan_lib.py:65-212): sample the generator in inference mode in batches
 of 64, run Inception on the samples, compute FID / IS / KID (and MS-SSIM on the first generated samples when a task asks
-for images).  Everything up to the [N,2048] statistics stays on the GPU; sample generation can be sharded across ranks
+for images, and the fractal dimension from every sample's distances to the first ones).  Everything up to the [N,2048] statistics stays on the GPU; sample generation can be sharded across ranks
 with a final all-reduce of the statistics."""
 import time
 
@@ -121,9 +121,10 @@ class _EvalBatchGraph(object):
     K.copy_(self.pool, pool)
     K.copy_(self.logits, logits)
 
-  def run_batches(self, rng, num_batches, keeper):
+  def run_batches(self, rng, num_batches, keeper, seed_distances=None):
     """Draws the latents of all batches first (same RNG order as the eager path: z then labels, batch by batch), ships
-    them to the device in one copy, then replays the graph back to back with no host synchronisation in between."""
+    them to the device in one copy, then replays the graph back to back with no host synchronisation in between.  The
+    seed distances of a batch are enqueued before the next replay overwrites its images."""
     g = self.gan
     zs, ls = [], []
     for _ in range(num_batches):
@@ -146,6 +147,8 @@ class _EvalBatchGraph(object):
       self.acc.n += self.b
       if self.images is not None:
         keeper.add(self.images)
+        if seed_distances is not None:
+          seed_distances.add(self.images, self.b, keeper)
       if self.acc.keep:     # device-side copies; one device->host transfer at finish()
         self.acc.acts.append(self.pool.t.clone())
         self.acc.logits.append(self.logits.t.clone())
@@ -170,6 +173,42 @@ class _ImageKeeper(object):
       return K.affine(tape.DT(torch.cat(self.parts)), 255.0)
 
 
+class _SeedDistances(object):
+  """The float64 distances of every generated sample of one averaging run to its first `s` samples, x255 (the fractal
+  dimension's seeds), measured batch by batch so that no image beyond the keeper's is retained.  The seeds are copied
+  out of the keeper once it holds them and the rows it holds are measured in one call; from then on each batch is
+  measured as it arrives."""
+
+  def __init__(self, s, image_shape, rows):
+    dev = K._RT["device"]
+    self.s, self.d = s, int(np.prod(image_shape))
+    self.seeds, self.parts, self.seen = None, [], 0
+    # one call on zeros sizes the library workspace for calls of up to `rows` rows now: it must not be reallocated once
+    # an evaluation graph has captured pointers into it
+    K.fd_distances(torch.zeros(rows, self.d, device=dev), torch.zeros(s, self.d, device=dev), 255.0)
+
+  def _measure(self, rows):
+    self.parts.append(K.fd_distances(rows.reshape(-1, self.d), self.seeds, 255.0))
+
+  def add(self, imgs, valid, keeper):
+    """imgs: the batch just generated (DT in [0, 1], its first `valid` rows count), after keeper.add(imgs, valid)."""
+    first = self.seen
+    self.seen += valid
+    if self.seeds is not None:
+      self._measure(imgs.t[:valid])
+    elif keeper.have >= self.s:
+      held = torch.cat(keeper.parts).reshape(keeper.have, self.d)
+      self.seeds = held[:self.s].clone()
+      self._measure(held)
+      in_keeper = keeper.have - first       # rows of this batch the keeper holds, measured with them
+      if in_keeper < valid:
+        self._measure(imgs.t[in_keeper:valid])
+
+  def finish(self):
+    """[n, s] float64 on the device, None when the run had fewer than s samples."""
+    return torch.cat(self.parts) if self.seeds is not None else None
+
+
 def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size=64, seed=42, num_accu_examples=204800,
              keep_features=True, real_images=None, use_graph=True, fuse_batches=4):
   """Mirrors evaluate_tfhub_module (reference eval_gan_lib.py:95-212).  Returns the result dict with
@@ -182,19 +221,22 @@ def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size
   K.sync_stream()
   fake_dsets, timings = [], []
   n_images = max([getattr(task, "images_needed", 0) for task in eval_tasks] + [0])
+  n_seeds = max([getattr(task, "distance_seeds", 0) for task in eval_tasks] + [0])
+  n_images = max(n_images, n_seeds)
   with use_ema_weights(gan):
     _update_bn_accumulators(gan, batch_size, num_accu_examples, rng)
     for _ in range(num_averaging_runs):
       acc = eval_utils.FeatureAccumulator(keep_features=keep_features)
       keeper = _ImageKeeper(n_images)
       fuse = max(1, min(int(fuse_batches), n_local // (4 * batch_size)))
+      seeds = _SeedDistances(n_seeds, dataset.image_shape, max(batch_size * fuse, n_images)) if n_seeds else None
       graph = _EvalBatchGraph(gan, batch_size, acc, fuse, n_images > 0) if (use_graph and n_local >= 4 * batch_size) else None
       torch.cuda.synchronize()
       t0 = time.time()
       done = 0
       if graph is not None:
         nb = n_local // (batch_size * fuse)
-        graph.run_batches(rng, nb, keeper)
+        graph.run_batches(rng, nb, keeper, seeds)
         done += nb * batch_size * fuse
       while done < n_local:
         imgs = generate_batch(gan, batch_size, rng)
@@ -202,10 +244,12 @@ def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size
         valid = min(batch_size, n_local - done)
         acc.add(pool, logits, valid)
         keeper.add(imgs, valid)
+        if seeds is not None:
+          seeds.add(imgs, valid, keeper)
         done += valid
       torch.cuda.synchronize()
       timings.append(time.time() - t0)
-      sample = acc.finish(eval_utils.EvalDataSample(keeper.images255()))
+      sample = acc.finish(eval_utils.EvalDataSample(keeper.images255(), None if seeds is None else seeds.finish()))
       if sample.activations is not None and not np.isfinite(sample.activations).all():
         raise eval_utils.NanFoundError("NaN in generated samples")
       fake_dsets.append(sample)

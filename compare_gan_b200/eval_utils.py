@@ -18,8 +18,11 @@ class EvalDataSample(object):
   FID moments accumulated on the device.  For a generated set `images` holds the first N samples (N = the largest
   images_needed of the evaluation's tasks, in [0, 255], on the device), not the whole set; None when no task needs them."""
 
-  def __init__(self, images=None):
+  def __init__(self, images=None, seed_distances=None):
     self._images = images
+    # [n, S] float64 on the device: the distances of the generated samples to the first S of them (x255), for the
+    # fractal dimension; None when no task needs them
+    self.seed_distances = seed_distances
     self.activations = None
     self.logits = None
     self.moments = None          # (mu, sigma) float64 from the device accumulator

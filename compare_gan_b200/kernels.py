@@ -793,6 +793,35 @@ def kmeans_finish(x, centroids, n_eval):
   return labels, inertia.cpu().numpy(), counts.cpu().numpy()
 
 
+def fd_distances(x, seeds, scale=1.0):
+  """float64 Euclidean distances of every row of x [n, d] to every seed [s, d] (metrics/fractal_dimension.py:67-68),
+  both fp32 torch tensors on the device, each value taken as fp32(scale * v).  Returns [n, s] float64 on the device."""
+  n, d = x.shape
+  s = seeds.shape[0]
+  assert seeds.shape[1] == d and x.is_contiguous() and seeds.is_contiguous()
+  out = torch.empty(n, s, dtype=torch.float64, device=_RT["device"])
+  _call("fd_distances", out.data_ptr(), x.data_ptr(), n, seeds.data_ptr(), s, d, float(scale))
+  return out
+
+
+def fd_range(dist):
+  """(smallest non-zero, largest) of a non-negative float64 device tensor, as numpy [2] (fractal_dimension.py:69-70);
+  the first is +inf when every value is 0."""
+  out = torch.empty(2, dtype=torch.float64, device=_RT["device"])
+  _call("fd_range", out.data_ptr(), dist.data_ptr(), dist.numel())
+  return out.cpu().numpy()
+
+
+def fd_counts(dist, edges):
+  """counts[j] = #{dist < edges[j]} for non-decreasing float64 edges (host values; fractal_dimension.py:78).  Returns
+  numpy int64 [len(edges)]."""
+  import numpy as np
+  e = torch.from_numpy(np.ascontiguousarray(edges, np.float64)).to(_RT["device"])
+  counts = torch.empty(e.numel(), dtype=torch.int64, device=_RT["device"])
+  _call("fd_counts", counts.data_ptr(), dist.data_ptr(), dist.numel(), e.data_ptr(), e.numel())
+  return counts.cpu().numpy()
+
+
 def globalpool(x, mean):
   """tf.reduce_mean / reduce_sum over axes [1,2] (resnet_cifar.py:156, resnet_biggan.py:405)."""
   n, h, w, c = x.shape

@@ -9,6 +9,9 @@ class EvalTask(object):
   # how many generated images (the first ones of each averaging run, x255, on the device) the task reads from
   # fake_dset.images; 0: none, and the evaluation keeps no images
   images_needed = 0
+  # how many seed samples (the first ones of each averaging run) the task needs the float64 distances of every generated
+  # sample to, in fake_dset.seed_distances [n, seeds]; 0: none, and the evaluation measures none
+  distance_seeds = 0
 
   def metric_list(self):
     return frozenset(self._LABEL)

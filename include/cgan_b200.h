@@ -327,6 +327,21 @@ int cgan_kmeans_lloyd_step(cgan_ctx*, double* centroids, int32_t* labels, int32_
 int cgan_kmeans_finish(cgan_ctx*, int32_t* labels, double* inertia, int32_t* counts, const double* centroids,
                        const float* x, int m, int d, int k, int groups, int n_eval);
 
+/* ---- fractal dimension (metrics/fractal_dimension.py:39-97) ---- */
+/* out [n, s] float64: out[i, j] = sqrt(sum_k (x'[i, k] - s'[j, k])^2) with x' = fp32(scale * x[i, k]) and
+ * s' = fp32(scale * seeds[j, k]) (x [n, d], seeds [s, d] fp32; scale = 255 gives the reference's float32 images * 255,
+ * eval_utils.py:157), each converted to float64 before the subtraction, the squares accumulated with a float64 FMA and
+ * the sqrt correctly rounded: the scipy.spatial.distance.cdist of fractal_dimension.py:67-68.  Direct differences, so
+ * a row equal to a seed is at distance exactly 0.  A row's bits depend on d only: not on n, on the other rows of the
+ * call or on the call's position in a run.  Workspace: partial sums of D slices, at most 64 MB. */
+int cgan_fd_distances(cgan_ctx*, double* out, const float* x, int n, const float* seeds, int s, int d, float scale);
+/* out2[0] = the smallest non-zero and out2[1] = the largest of dist[0, count) (non-negative values), exact
+ * (fractal_dimension.py:69-70); out2[0] = +inf when every value is 0, and out2[1] is NaN when one is. */
+int cgan_fd_range(cgan_ctx*, double* out2, const double* dist, int64_t count);
+/* counts[j] = #{q < count : dist[q] < edges[j]} for non-decreasing edges [nedges] in device memory (1 <= nedges <= 8192):
+ * np.sum(np.less.outer(dist, edges), axis=0) of fractal_dimension.py:78, exact (integer histogram + prefix sum). */
+int cgan_fd_counts(cgan_ctx*, int64_t* counts, const double* dist, int64_t count, const double* edges, int nedges);
+
 /* ---- cross-replica exchange of small vectors (tpu/tpu_ops.py:75-125: cross_replica_mean / cross_replica_moments) ---- */
 /* One process per GPU on one node.  Every rank allocates a communication buffer and publishes its cudaIpc handle
  * (cgan_p2p_local_handle -> 64 bytes), the host code all-gathers the handles (torch.distributed) and hands all of them
