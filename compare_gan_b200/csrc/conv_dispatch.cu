@@ -305,5 +305,7 @@ int cgan_gemm_batched(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float 
 
 int cgan_gemm(cgan_ctx* ctx, int ta, int tb, int m, int n, int k, float alpha, const float* a, int lda, const float* b,
               int ldb, float beta, float* c, int ldc) {
+  if (!ctx) return CGAN_ERR_ARG;
+  ctx->last_path = CGAN_PATH_SIMT_FP32;
   return cgan_gemm_batched_simt(ctx, ta, tb, m, n, k, alpha, a, lda, 0, b, ldb, 0, beta, c, ldc, 0, 1);
 }

@@ -50,7 +50,7 @@ int64_t cgan_launch_count(cgan_ctx* ctx);
  *                       kh*kw*channels <= 32: every discriminator's first and every generator's last convolution, Inception's
  *                       stem) run as ONE 32-wide GEMM on the tensor-core kernels over a [pixels, 32] patch tensor (csrc/thin_tc.cu),
  *                       TF32 operands like every other tensor-core contraction; 0: the exact-fp32 streaming kernels (thin.cu).
- *   CGAN_OPT_LAST_PATH  (get) CGAN_PATH_* taken by the most recent conv2d_fwd / dgrad / wgrad / gemm_batched call.
+ *   CGAN_OPT_LAST_PATH  (get) CGAN_PATH_* taken by the most recent conv2d_fwd / dgrad / wgrad / gemm / gemm_batched call.
  *   CGAN_OPT_LAST_TC_BN, CGAN_OPT_LAST_TC_MT, CGAN_OPT_LAST_TC_HALO
  *                       (get) column-tile width, pixel tiles per CTA and halo kernel (1) or per-tap kernel (0) of the most
  *                       recent tensor-core convolution kernel launch (the wgmma implicit GEMM, not the filter gradient);
