@@ -649,14 +649,16 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
     return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(B) failed%s", "cgan_conv_tc");
 
   // Pixel tiles per CTA: with mt = 2 the weight tile is fetched once for 256 pixels, which cuts the L2->SM bytes per MMA
-  // by a third; the accumulators (mt x bn columns) must fit the consumer registers, so only for bn <= 128, and only when
-  // enough CTAs remain to fill the machine.  Up to ~110 KB of smem per CTA when the tile is narrow, so that two CTAs
-  // share an SM and one's epilogue overlaps the other's main loop.
+  // by a third; only when enough CTAs remain to fill the machine.  Up to ~110 KB of smem per CTA when mt x bn <= 128, so
+  // that two CTAs share an SM and one's epilogue overlaps the other's main loop.  That overlap is worth more than the
+  // bytes: on H100 a 128-column tile at mt = 1 (two CTAs per SM) runs the 3x3 128->128 conv at 32x32, batch 512, in
+  // 0.97 ms against 1.39 ms at mt = 2 (one CTA per SM, the register file holds one 256-column accumulator set).  So
+  // mt = 2 only where two such CTAs still share an SM: bn <= 64.
   const long long tiles_total = (long long)p.tiles_w * p.tiles_h * tiles_n;
   const int ncol_tiles = ncols_pad / p.bn;
   p.tiles_total = (int)tiles_total;
   p.mt = 1;
-  if (ctx->tc_mt_max >= 2 && 2 * p.bn <= TC_ACC_COLS && tiles_total * ncol_tiles * p.nphases >= 4ll * ctx->num_sms &&
+  if (ctx->tc_mt_max >= 2 && 2 * p.bn <= 128 && tiles_total * ncol_tiles * p.nphases >= 4ll * ctx->num_sms &&
       (c.wimg_stride == 0 || (p.tiles_w * p.tiles_h) % 2 == 0))
     p.mt = 2;
   const bool two_ctas = p.mt * p.bn <= 128;

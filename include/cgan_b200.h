@@ -42,7 +42,8 @@ const char* cgan_last_error(cgan_ctx* ctx);
 int64_t cgan_launch_count(cgan_ctx* ctx);
 /* Tuning knobs and introspection (tests compare kernel variants bit for bit and ask which path a contraction took).
  *   CGAN_OPT_TC_MT      (set/get) max pixel tiles (conv) / work units (filter gradient) per tensor-core CTA: 1 or 2
- *                       (2 only where the accumulators of both fit the registers: column tiles <= 128 wide).
+ *                       (2 only where it pays: convolution column tiles <= 64 wide, so that two CTAs still share an SM;
+ *                       filter-gradient column tiles <= 128 wide, where the accumulators of both fit the registers).
  *   CGAN_OPT_TC_HALO    (set/get) 3x3 stride-1 tensor-core convolutions fetch one (rows+2)-row activation box per kernel
  *                       column instead of one box per tap: 0 never, 1 where the operand is rounded in the kernel and there
  *                       are >= 256 output channels (default), 2 wherever the geometry allows.
