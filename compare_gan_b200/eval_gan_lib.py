@@ -1,6 +1,7 @@
 """Evaluation of a trained GAN (reference eval_gan_lib.py:65-212): sample the generator in inference mode in batches
 of 64, run Inception on the samples, compute FID / IS / KID (and MS-SSIM on the first generated samples when a task asks
-for images, and the fractal dimension from every sample's distances to the first ones).  Everything up to the [N,2048] statistics stays on the GPU; sample generation can be sharded across ranks
+for images, the fractal dimension from every sample's distances to the first ones, and the metric tensors of G's
+Jacobian for the condition number).  Everything up to the [N,2048] statistics stays on the GPU; sample generation can be sharded across ranks
 with a final all-reduce of the statistics."""
 import time
 
@@ -223,9 +224,10 @@ def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size
   n_images = max([getattr(task, "images_needed", 0) for task in eval_tasks] + [0])
   n_seeds = max([getattr(task, "distance_seeds", 0) for task in eval_tasks] + [0])
   n_images = max(n_images, n_seeds)
+  n_cond = max([getattr(task, "condition_samples", 0) for task in eval_tasks] + [0])
   with use_ema_weights(gan):
     _update_bn_accumulators(gan, batch_size, num_accu_examples, rng)
-    for _ in range(num_averaging_runs):
+    for run in range(num_averaging_runs):
       acc = eval_utils.FeatureAccumulator(keep_features=keep_features)
       keeper = _ImageKeeper(n_images)
       fuse = max(1, min(int(fuse_batches), n_local // (4 * batch_size)))
@@ -250,6 +252,12 @@ def evaluate(gan, eval_tasks, num_averaging_runs=1, num_samples=None, batch_size
       torch.cuda.synchronize()
       timings.append(time.time() - t0)
       sample = acc.finish(eval_utils.EvalDataSample(keeper.images255(), None if seeds is None else seeds.finish()))
+      if n_cond and rank == 0:
+        # the G that FID saw (EMA weights, filled accumulators), with latents of its own stream; after this run's graph is
+        # done with and before the next one is captured (the pass may grow the library workspace)
+        from .metrics import jacobian_conditioning
+        sample.metric_tensors = jacobian_conditioning.generator_metric_tensors(
+            gan, n_cond, np.random.RandomState(seed + 7919 * (run + 1)))
       if sample.activations is not None and not np.isfinite(sample.activations).all():
         raise eval_utils.NanFoundError("NaN in generated samples")
       fake_dsets.append(sample)

@@ -23,6 +23,9 @@ class EvalDataSample(object):
     # [n, S] float64 on the device: the distances of the generated samples to the first S of them (x255), for the
     # fractal dimension; None when no task needs them
     self.seed_distances = seed_distances
+    # [n, z_dim, z_dim] float64 (numpy): the metric tensors of G's Jacobian at n latent samples, for the generator
+    # condition number; None when no task needs them
+    self.metric_tensors = None
     self.activations = None
     self.logits = None
     self.moments = None          # (mu, sigma) float64 from the device accumulator

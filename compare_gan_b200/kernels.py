@@ -9,6 +9,7 @@ BN / attention) raises NotImplementedError instead of silently dropping the seco
 These are the H100 stand-ins for the TF library calls the reference's ops library makes
 (arch_ops.py / resnet_ops.py / loss_lib.py / penalty_lib.py); file:line citations sit on each op.
 """
+import contextlib
 import ctypes
 
 import torch
@@ -141,6 +142,79 @@ def _call(name, *args):
   _RT["lib"].call(name, *args)
 
 
+# ------------------------------------------------------------------------------------ forward mode
+# The generator-conditioning metric (metrics/jacobian_conditioning.py) needs the Jacobian of G w.r.t. z: k = z_dim
+# tangent columns pushed forward through the ops G reaches in inference mode.  A tensor's tangents live in DT.tan,
+# [rows * k, ...] sample-major (tape.DT); an op with a rule below sets its output's tangent whenever an input carries one.
+# Linear ops run their own kernel on the tangent batch (weights, biases, spectral norm, label embeddings and BN moments are
+# constants of the pass); nonlinear ops read their primal once per tangent (csrc/jacobian.cu).  An op without a rule
+# raises (tape.attach, _constant) instead of dropping a tangent.
+
+_FWD = [None]     # (samples, k) of the running forward-mode pass
+
+
+@contextlib.contextmanager
+def forward_mode(samples, k):
+  """Tangents of `samples` primal samples, k per sample, may flow through the ops inside this scope."""
+  _FWD.append((int(samples), int(k)))
+  try:
+    yield
+  finally:
+    _FWD.pop()
+
+
+def _tk(x):
+  """(tangent of x, k), (None, 0) without one."""
+  t = None if x is None else x.tan
+  if t is None:
+    return None, 0
+  if _FWD[-1] is None:
+    raise RuntimeError("a tensor carries tangents outside kernels.forward_mode")
+  return t, _FWD[-1][1]
+
+
+def _constant(name, *xs):
+  """Operands that are constants of a forward-mode pass (weights, statistics) or inputs of an op without a rule."""
+  for x in xs:
+    if x is not None and getattr(x, "tan", None) is not None:
+      raise NotImplementedError("forward-mode tangents through %s are not implemented for this operand" % name)
+
+
+def _desc_times(d, k):
+  """The convolution `d` over k times as many images (the tangent batch)."""
+  return _lib.ConvDesc(d.n * k, d.h, d.w, d.cin, d.cout, d.kh, d.kw, d.stride, d.upsample, d.oh, d.ow, d.pad_t, d.pad_l)
+
+
+def act_jvp(t, ref, kind, leak=0.0):
+  """t * act'(ref) with ref (x for relu / lrelu, y for sigmoid / tanh01) broadcast over the k tangents of each sample."""
+  samples, k = _FWD[-1]
+  out = empty(*t.shape)
+  _call("act_jvp", out.ptr, t.ptr, ref.ptr, int(kind), float(leak), samples, ref.numel // samples, k)
+  return out
+
+
+def bn_apply_jvp(t_x, x, mean_var, eps, gamma, t_gamma, t_beta, cond, y_relu=None):
+  """Tangent of bn_apply with the moments constant; y_relu: the primal output of a fused ReLU (its mask)."""
+  samples, k = _FWD[-1]
+  c = x.shape[-1]
+  rows = x.numel // c
+  out = empty(rows * k, c)
+  _call("bn_apply_jvp", out.ptr, None if t_x is None else t_x.ptr, x.ptr, None if y_relu is None else y_relu.ptr, rows, c,
+        rows // samples, mean_var.ptr, float(eps), None if gamma is None else gamma.ptr,
+        None if t_gamma is None else t_gamma.ptr, None if t_beta is None else t_beta.ptr, int(cond), k)
+  return out.view((x.shape[0] * k,) + tuple(x.shape[1:]))
+
+
+def metric_tensor_f64(tangents):
+  """M[b] = T[b] T[b]^T in float64 for the fp32 tangent output T [B, k, D] (a torch tensor on the device), as a
+  [B, k, k] float64 device tensor (jacobian_conditioning.py:146-173)."""
+  b, k, d = tangents.shape
+  assert tangents.dtype == torch.float32 and tangents.is_contiguous()
+  m = torch.empty(b, k, k, dtype=torch.float64, device=tangents.device)
+  _call("metric_tensor_f64", m.data_ptr(), tangents.data_ptr(), b, k, d)
+  return m
+
+
 # ------------------------------------------------------------------------------------ basic helpers
 
 def _grad_out(leaf, *shape):
@@ -175,6 +249,9 @@ def reshape(x, *shape):
   """tf.reshape: zero-copy view, taped."""
   y = DT(x.t.view(*shape))
   y.tf32 = x.tf32
+  t, k = _tk(x)
+  if t is not None:
+    y.tan = t.view(y.shape[0] * k, *y.shape[1:])
   xs = x.shape
   return attach("reshape", y, [x], lambda g, needs: [reshape(g, *xs)])
 
@@ -185,6 +262,10 @@ def add(a, b, round_tf32=False):
   rnd = bool(round_tf32) and tf32_on()
   _call("add_tf32", y.ptr, a.ptr, b.ptr, y.numel, int(rnd))
   y.tf32 = rnd
+  ta, _ = _tk(a)
+  tb, _ = _tk(b)
+  if ta is not None or tb is not None:
+    y.tan = ta if tb is None else (tb if ta is None else add(ta, tb))
   return attach("add", y, [a, b], lambda g, needs: [g if needs[0] else None, g if needs[1] else None])
 
 
@@ -293,6 +374,11 @@ def concat_cols(a, b):
   y = empty(n, ca + cb)
   _call("copy2d", y.ptr, ca + cb, 0, a.ptr, ca, 0, n, ca)
   _call("copy2d", y.ptr, ca + cb, ca, b.ptr, cb, 0, n, cb)
+  ta, ka = _tk(a)
+  tb, kb = _tk(b)
+  if ta is not None or tb is not None:
+    k = ka or kb
+    y.tan = concat_cols(ta if ta is not None else zeros(n * k, ca), tb if tb is not None else zeros(n * k, cb))
 
   def vjp(g, needs):
     return [slice_cols(g, 0, ca) if needs[0] else None, slice_cols(g, ca, ca + cb) if needs[1] else None]
@@ -304,6 +390,9 @@ def slice_cols(x, lo, hi):
   n, c = x.shape
   y = empty(n, hi - lo)
   _call("copy2d", y.ptr, hi - lo, 0, x.ptr, c, lo, n, hi - lo)
+  t, _ = _tk(x)
+  if t is not None:
+    y.tan = slice_cols(t, lo, hi)
 
   def vjp(g, needs):
     full = zeros(n, c)
@@ -356,6 +445,7 @@ def conv2d_relu(x, w, bias, stride=1, padding="SAME", sink=None, sink_off=0):
   """relu(conv2d(x, w) + bias) in one kernel; inference only (no tape).  With `sink` (a ChannelSink) the result is
   stored straight into channels [sink_off, sink_off + cout) of the wider NHWC tensor (tf.concat(axis=3) without the
   copy) and None is returned."""
+  _constant("conv2d_relu", x)
   n, h, ww, cin = x.shape
   kh, kw, _, cout = w.shape
   d = conv_desc(n, h, ww, cin, cout, kh, kw, stride, False, padding)
@@ -411,6 +501,12 @@ def conv2d(x, w, bias=None, stride=1, upsample=False, padding="SAME", relu=False
   yv = DT(y.t) if relu else None        # y > 0  <=>  pre-activation > 0
   if relu:
     y.relu_of = (yv, 0.0)
+  tx, kx = _tk(x)
+  tr, kr = _tk(residual)
+  if tx is not None or tr is not None:
+    _constant("conv2d", w, bias)
+    t = tr if tx is None else _conv_fwd_raw(_desc_times(d, kx), tx, w, None, residual=tr)
+    y.tan = act_jvp(t, yv, ACT_RELU) if relu else t
   y_id = id(y)
 
   def vjp(g, needs):
@@ -438,6 +534,14 @@ def conv2d_dgrad(d, dy, w, bias=None, round_out=False, relu_mask=None, mask_for=
     dx.premasked_for = id(mask_for)
   if CONV_CHECK is not None:
     CONV_CHECK("dgrad", d=d, dy=dy, w=w, bias=bias, round_out=rnd, mask=mref, mask_leak=mleak, out=dx, arith=_arith(dy.tf32))
+  tdy, k = _tk(dy)
+  if tdy is not None:                    # the transposed convolution of a generator (deconv2d)
+    _constant("conv2d_dgrad", w, bias)
+    if mref is not None:
+      raise NotImplementedError("forward-mode tangents through a masked conv2d_dgrad are not implemented")
+    dt = _desc_times(d, k)
+    dx.tan = empty(dt.n, d.h, d.w, d.cin)
+    _call("conv2d_dgrad_ex", ctypes.byref(dt), tdy.ptr, w.ptr, ctypes.byref(_epilogue()), dx.tan.ptr)
   cin = d.cin
 
   def vjp(g, needs):   # linear in dy and in w
@@ -497,6 +601,12 @@ def matmul(a, b, ta=False, tb=False, leaf=None):
     raise ValueError("matmul: inner dimensions differ: %d vs %d" % (k, kb))
   c = _grad_out(leaf, m, n)
   _call("gemm", int(ta), int(tb), m, n, k, 1.0, a.ptr, a.shape[1], b.ptr, b.shape[1], 0.0, c.ptr, n)
+  t, _ = _tk(a)
+  if t is not None:                      # z-dependent rows times a constant weight (linear)
+    _constant("matmul", b)
+    if ta:
+      raise NotImplementedError("forward-mode tangents through a transposed matmul operand are not implemented")
+    c.tan = matmul(t, b, False, tb)
 
   def vjp(g, needs):
     ga = gb = None
@@ -520,6 +630,10 @@ def bmm(a, b, ta=False, tb=False):
   _trace("bmm", (bsz, int(ta), int(tb), m, n, k))
   if CONV_CHECK is not None:
     CONV_CHECK("bmm", a=a, b=b, ta=ta, tb=tb, out=c, arith=_arith())
+  t_a, ka = _tk(a)
+  t_b, kb = _tk(b)
+  if t_a is not None or t_b is not None:
+    c.tan = _bmm_jvp(a, b, t_a, t_b, ta, tb, ka or kb, m, n, k)
 
   def vjp(g, needs):
     ga = gb = None
@@ -529,6 +643,23 @@ def bmm(a, b, ta=False, tb=False):
       gb = bmm(g, a, True, ta) if tb else bmm(a, g, not ta, False)
     return [ga, gb]
   return attach("bmm", c, [a, b], vjp)
+
+
+def _bmm_jvp(a, b, t_a, t_b, ta, tb, kt, m, n, kd):
+  """Product rule of bmm: t_c = t_a b + a t_b, per sample one batched GEMM over its kt tangents for each term, the
+  sample's primal operand read with batch stride 0."""
+  bsz = a.shape[0]
+  sa, sb, sc = a.shape[1] * a.shape[2], b.shape[1] * b.shape[2], m * n
+  out = empty(bsz * kt, m, n)
+  for s in range(bsz):
+    o = out.ptr + 4 * s * kt * sc
+    if t_a is not None:
+      _call("gemm_batched", int(ta), int(tb), m, n, kd, 1.0, t_a.ptr + 4 * s * kt * sa, a.shape[2], sa,
+            b.ptr + 4 * s * sb, b.shape[2], 0, 0.0, o, n, sc, kt)
+    if t_b is not None:
+      _call("gemm_batched", int(ta), int(tb), m, n, kd, 1.0, a.ptr + 4 * s * sa, a.shape[2], 0,
+            t_b.ptr + 4 * s * kt * sb, b.shape[2], sb, 1.0 if t_a is not None else 0.0, o, n, sc, kt)
+  return out
 
 
 def round_tf32(x):
@@ -559,6 +690,7 @@ def attention(theta, phi, g):
   ops are composed as the reference writes them."""
   if not attention_fused_ok(theta, phi, g):
     return bmm(softmax(bmm(theta, phi, False, True)), g)
+  _constant("the fused attention kernel (math_mode 1)", theta, phi, g)
   bsz, lq, dk = theta.shape
   lk, dv = g.shape[1], g.shape[2]
   q, k, v = round_tf32(theta), round_tf32(phi), round_tf32(g)
@@ -586,6 +718,7 @@ def attention(theta, phi, g):
 
 def colsum(x2, groups=1, leaf=None):
   """Per-channel sum over rows (bias / beta gradients).  `leaf`: the variable this is the gradient of, see _grad_out."""
+  _constant("colsum", x2)
   rows, c = x2.shape
   out = _grad_out(leaf, c) if groups == 1 else empty(groups, c)
   _call("colsum", out.ptr, x2.ptr, groups, rows // groups, c)
@@ -596,6 +729,10 @@ def bias_add(x, bias):
   c = x.shape[-1]
   y = empty(*x.shape)
   _call("bias_add", y.ptr, x.ptr, bias.ptr, x.numel // c, c)
+  t, _ = _tk(x)
+  if t is not None:
+    _constant("bias_add", bias)
+    y.tan = t
 
   def vjp(g, needs):
     return [g if needs[0] else None, colsum(reshape(g, -1, c), leaf=bias) if needs[1] else None]
@@ -622,6 +759,9 @@ def act(x, kind, leak=0.0, round_tf32=False):
   ref = x if kind in (ACT_RELU, ACT_LRELU) else DT(y.t)
   if kind in (ACT_RELU, ACT_LRELU):
     y.relu_of = (DT(x.t), float(leak) if kind == ACT_LRELU else 0.0)
+  t, _ = _tk(x)
+  if t is not None:
+    y.tan = act_jvp(t, ref, kind, leak)
   y_id = id(y)
 
   def vjp(g, needs):
@@ -666,6 +806,9 @@ def avgpool2(x):
   n, h, w, c = x.shape
   y = empty(n, h // 2, w // 2, c)
   _call("avgpool2_fwd", y.ptr, x.ptr, n, h, w, c)
+  t, _ = _tk(x)
+  if t is not None:
+    y.tan = avgpool2(t)
   return attach("avgpool2", y, [x], lambda g, needs: [avgpool2_bwd(g, h, w)])
 
 
@@ -687,6 +830,10 @@ def unpool(x):
   x / 4 over each 2x2 cell, a per-pixel scale (4 at the even-even pixel, 0 elsewhere) keeps the corner — exact in fp32,
   and differentiable to any order because both parts are taped ops."""
   import numpy as np
+  if x.tan is not None:                 # linear: the tangent is the unpooled tangent batch (inference only, no tape)
+    y = unpool(DT(x.t))
+    y.tan = unpool(x.tan)
+    return y
   n, h, w, c = x.shape
   key = (n, h, w, str(_RT["device"]))
   if key not in _UNPOOL_MASKS:          # built once per shape, i.e. during the eager warm-up that precedes graph capture
@@ -703,6 +850,10 @@ def maxpool2(x):
   y = empty(n, h // 2, w // 2, c)
   _call("maxpool2_fwd", y.ptr, x.ptr, n, h, w, c)
   y.tf32 = x.tf32           # a maximum of TF32 values is one of them
+  t, k = _tk(x)
+  if t is not None:
+    y.tan = empty(n * k, h // 2, w // 2, c)
+    _call("maxpool2_jvp", y.tan.ptr, t.ptr, x.ptr, n, h, w, c, k)
 
   def vjp(g, needs):
     _no_second_order("maxpool2")
@@ -714,6 +865,7 @@ def maxpool2(x):
 
 def pool2d(x, k, stride, padding, mode):
   """tf.nn.max_pool / tf.nn.avg_pool (TF-GAN's Inception graph); inference only."""
+  _constant("pool2d", x)
   n, h, w, c = x.shape
   if padding == "SAME":
     oh, pt = same_pad(h, k, stride)
@@ -727,6 +879,7 @@ def pool2d(x, k, stride, padding, mode):
 
 def concat_channels(xs):
   """tf.concat(axis=3) of NHWC tensors (Inception mixed blocks); inference only."""
+  _constant("concat_channels", *xs)
   n, h, w = xs[0].shape[:3]
   ctot = sum(t.shape[3] for t in xs)
   y = empty(n, h, w, ctot)
@@ -740,6 +893,7 @@ def concat_channels(xs):
 
 def resize_bilinear(x, oh, ow, inception_scale=False):
   """tf.image.resize_bilinear (align_corners=False); with inception_scale also (v*255-128)/128 (eval_utils.py:157-175)."""
+  _constant("resize_bilinear", x)
   n, h, w, c = x.shape
   y = empty(n, oh, ow, c)
   _call("resize_bilinear", y.ptr, x.ptr, n, h, w, c, oh, ow, 1 if inception_scale else 0)
@@ -851,6 +1005,11 @@ def softmax(x):
   y = empty(*shape)
   _call("softmax_fwd", y.ptr, x.ptr, rows, cols)
   yv = DT(y.t)
+  t, k = _tk(x)
+  if t is not None:                      # the softmax Jacobian is symmetric: the tangent is softmax_bwd(t, y)
+    samples = _FWD[-1][0]
+    y.tan = empty(*((shape[0] * k,) + tuple(shape[1:])))
+    _call("softmax_jvp", y.tan.ptr, t.ptr, y.ptr, samples, rows // samples, cols, k)
 
   def vjp(g, needs):
     _no_second_order("softmax")
@@ -881,6 +1040,11 @@ def scale_by_param(x, s):
   """x * s with s a scalar parameter on device (non_local_block sigma, arch_ops.py:755-758)."""
   y = empty(*x.shape)
   _call("scale_by_dev", y.ptr, x.ptr, s.ptr, 1.0, 0, y.numel)
+  t, _ = _tk(x)
+  if t is not None:
+    _constant("scale_by_param", s)
+    y.tan = empty(*t.shape)
+    _call("scale_by_dev", y.tan.ptr, t.ptr, s.ptr, 1.0, 0, t.numel)
 
   def vjp(g, needs):
     _no_second_order("scale_by_param")
@@ -905,6 +1069,7 @@ def one_hot(labels_i32, classes):
 
 def interpolate(x, xf, alpha):
   """x + alpha*(x_fake - x), alpha [B,1,1,1] (penalty_lib.py:74-75).  Result is a fresh leaf."""
+  _constant("interpolate", x, xf)
   y = empty(*x.shape)
   _call("interpolate", y.ptr, x.ptr, xf.ptr, alpha.ptr, x.shape[0], x.numel // x.shape[0])
   return y
@@ -928,6 +1093,7 @@ def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_afte
   gamma/beta: [C] DTs, or [N,C] when cond (conditional BN); either may be None.
   allreduce(stats_dt) sums a [2C] buffer over replicas (cross-replica moments, tpu_ops.py:94-125).
   """
+  _constant("bn_train", x, gamma, beta)
   c = x.shape[-1]
   rows = x.numel // c
   rps = rows // x.shape[0]
@@ -1005,6 +1171,14 @@ def bn_infer(x, gamma, beta, eps, state, use_moving_averages, cond=False, relu_a
   _call("bn_apply", y.ptr, x.ptr, rows, c, rps, mv.ptr, float(eps), None if gamma is None else gamma.ptr,
         None if beta is None else beta.ptr, int(cond), (1 if relu_after else 0) | (_lib.ACT_ROUND_TF32 if rnd else 0))
   y.tf32 = rnd
+  tx, _ = _tk(x)
+  tg, _ = _tk(gamma)
+  tb, _ = _tk(beta)
+  if tx is not None or tg is not None or tb is not None:
+    if not cond:
+      _constant("bn_infer (an unconditional gamma / beta)", gamma, beta)
+    # BigGAN's conditional gamma / beta depend on z through the hierarchical chunks; the moments are constants
+    y.tan = bn_apply_jvp(tx, x, mv, eps, gamma, tg, tb, cond, y if relu_after else None)
   return y
 
 

@@ -12,6 +12,9 @@ class EvalTask(object):
   # how many seed samples (the first ones of each averaging run) the task needs the float64 distances of every generated
   # sample to, in fake_dset.seed_distances [n, seeds]; 0: none, and the evaluation measures none
   distance_seeds = 0
+  # how many latent samples the task needs the float64 metric tensors J^T J of G's Jacobian at, in
+  # fake_dset.metric_tensors [n, z_dim, z_dim]; 0: none, and the evaluation computes none
+  condition_samples = 0
 
   def metric_list(self):
     return frozenset(self._LABEL)

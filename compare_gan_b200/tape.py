@@ -16,7 +16,7 @@ import torch
 
 class DT(object):
   """Device tensor: float32 (or int32 labels), C-contiguous; 4-D tensors are NHWC."""
-  __slots__ = ("t", "node", "req", "tf32", "relu_of", "premasked_for", "__weakref__")
+  __slots__ = ("t", "node", "req", "tf32", "relu_of", "premasked_for", "tan", "__weakref__")
 
   def __init__(self, t, req=False):
     assert t.is_contiguous()
@@ -31,6 +31,9 @@ class DT(object):
     # premasked_for = id(tensor) marks a gradient that already carries that tensor's mask (kernels.conv2d_dgrad)
     self.relu_of = None
     self.premasked_for = None
+    # forward mode (metrics/jacobian_conditioning.py): a DT [shape[0] * k, ...] holding k tangents of every sample of this
+    # tensor, sample-major (row block b * k + j is tangent j of sample b); None when this tensor carries no tangent
+    self.tan = None
 
   @property
   def shape(self):
@@ -93,7 +96,10 @@ def recording():
 
 
 def attach(name, out, inputs, vjp):
-  """Record `out = op(inputs)`; vjp(gout, needs) -> list of grads (None where not needed)."""
+  """Record `out = op(inputs)`; vjp(gout, needs) -> list of grads (None where not needed).  An op that has a forward-mode
+  rule sets out.tan before it attaches; one that does not must never drop an input's tangent silently."""
+  if out.tan is None and any(i is not None and i.tan is not None for i in inputs):
+    raise NotImplementedError("forward-mode tangents through %s are not implemented" % name)
   if _RECORD[-1] and any(i is not None and i.req for i in inputs):
     out.req = True
     out.node = Node(name, inputs, vjp, out)

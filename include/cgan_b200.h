@@ -343,6 +343,34 @@ int cgan_fd_range(cgan_ctx*, double* out2, const double* dist, int64_t count);
  * np.sum(np.less.outer(dist, edges), axis=0) of fractal_dimension.py:78, exact (integer histogram + prefix sum). */
 int cgan_fd_counts(cgan_ctx*, int64_t* counts, const double* dist, int64_t count, const double* edges, int nedges);
 
+/* ---- generator conditioning (metrics/jacobian_conditioning.py:32-173) ---- */
+/* Forward-mode tangents of the generator's nonlinear ops.  A tangent batch holds k tangents per primal sample,
+ * sample-major: for n_primal samples of `per` values each, t[(s * k + j) * per + e] is tangent j of value e of sample s,
+ * and the primal (ref / x / y / p) is read once per tangent: t_out = t_in * act'(ref), with ref = x for relu / lrelu (mask
+ * ref > 0, else 0 / leak) and ref = y for sigmoid / tanh01, as cgan_act_bwd (arch_ops.py:595-597, sndcgan.py:74-78). */
+int cgan_act_jvp(cgan_ctx*, float* t_out, const float* t_in, const float* ref, int kind, float leak, int n_primal,
+                 int64_t per, int k);
+/* Tangent of cgan_bn_apply with the moments constant (arch_ops.py:66-191, 423-445): r = rsqrt(var + eps),
+ * xhat = (x - mean) r, t_y = t_x r gamma + xhat t_gamma + t_beta, then zero where y <= 0 when y (the primal output of a
+ * fused ReLU) is given.  x [rows, c] primal, rows_per_sample rows per sample; t_x / t_y [rows * k, c]; gamma [c]
+ * (cond = 0) or [rows / rows_per_sample, c] (cond = 1), nullable; t_gamma / t_beta [rows / rows_per_sample * k, c],
+ * cond = 1 only, nullable; t_x nullable (a zero tangent). */
+int cgan_bn_apply_jvp(cgan_ctx*, float* t_y, const float* t_x, const float* x, const float* y, int64_t rows, int c,
+                      int64_t rows_per_sample, const float* mean_var2c, float eps, const float* gamma, const float* t_gamma,
+                      const float* t_beta, int cond, int k);
+/* Tangent of cgan_maxpool2_fwd (arch_ops.py:741, 750): the tangent at the first maximum of the primal window. */
+int cgan_maxpool2_jvp(cgan_ctx*, float* t_out, const float* t_in, const float* x, int n_primal, int h, int w, int c, int k);
+/* Tangent of cgan_softmax_fwd (arch_ops.py:745): t_out = p (t_in - <t_in, p>) per row, which is cgan_softmax_bwd with
+ * the primal probabilities p [n_primal * rows_per_sample, cols] broadcast over the k tangents of each sample. */
+int cgan_softmax_jvp(cgan_ctx*, float* t_out, const float* t_in, const float* p, int n_primal, int64_t rows_per_sample,
+                     int cols, int k);
+/* Metric tensors M[b] = T[b] T[b]^T (jacobian_conditioning.py:146-173; there a float32 np.matmul) in float64: T [B, k, D]
+ * fp32 (the tangent output of B samples, k tangents each), M [B, k, k] float64.  The fp32 values are converted exactly,
+ * products are formed on the FP64 tensor cores and summed over fixed D slices in a fixed order: reruns are
+ * bit-identical, a sample's result does not depend on B, and M[b] is exactly symmetric.  Workspace: slice sums, at most
+ * 64 MB (or one sample's). */
+int cgan_metric_tensor_f64(cgan_ctx*, double* M, const float* T, int B, int k, int64_t D);
+
 /* ---- cross-replica exchange of small vectors (tpu/tpu_ops.py:75-125: cross_replica_mean / cross_replica_moments) ---- */
 /* One process per GPU on one node.  Every rank allocates a communication buffer and publishes its cudaIpc handle
  * (cgan_p2p_local_handle -> 64 bytes), the host code all-gathers the handles (torch.distributed) and hands all of them
