@@ -65,8 +65,7 @@ class AbstractDiscriminator(_Network):
   """images (and one-hot y) -> (probability, logit, penultimate features)."""
 
   def __init__(self, name="discriminator", batch_norm_fn=None, layer_norm=False, spectral_norm=False):
-    if layer_norm:
-      raise NotImplementedError("layer_norm is outside the accelerated hot path (SURVEY.md §2.1)")
+    # read by the residual-block discriminators (resnet_ops / resnet_biggan); the others ignore it, as the reference's do
     self._setup(name, batch_norm_fn, spectral_norm)
     self._layer_norm = layer_norm
 

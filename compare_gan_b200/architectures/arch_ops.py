@@ -186,6 +186,17 @@ def norm_relu(norm_fn, inputs, _tf32=False, **kwargs):
   return K.relu(norm_fn(inputs, **kwargs), round_tf32=_tf32)
 
 
+def layer_norm(inputs, is_training, scope, _relu=False, _tf32=False):
+  """tf.contrib.layers.layer_norm(inputs, trainable=is_training, scope=scope) (reference arch_ops.py:448-450): moments
+  per sample over H, W and C, beta / gamma per channel (created in that order, zeros / ones).  `_relu` fuses the
+  following ReLU, `_tf32` as in norm_relu."""
+  with V.variable_scope(scope):
+    c = inputs.shape[-1]
+    beta = V.get_variable("beta", (c,), zeros_init, trainable=is_training)
+    gamma = V.get_variable("gamma", (c,), ones_init, trainable=is_training)
+  return K.layer_norm(inputs, gamma, beta, relu_after=_relu, round_out=_tf32)
+
+
 # ----------------------------------------------------------------------------- spectral norm
 
 @gin.configurable(blacklist=["inputs"])

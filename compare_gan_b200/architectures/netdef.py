@@ -111,16 +111,27 @@ def _block_conv(x, plan, cin, cout, scale, suffix, kernel, use_sn, pool=True, **
   return K.avgpool2(y) if (scale == "down" and pool) else y
 
 
-def residual_block(inputs, plan, batch_norm, z, y, is_training, use_sn):
+def _norm_relu(batch_norm, layer_norm, x, idx, tf32, norm_kw):
+  """bn<idx> [-> ln<idx>] -> relu (resnet_ops.py:162-174, resnet_biggan.py:123-134), the ReLU fused into the last
+  normaliser."""
+  if not layer_norm:
+    return ops.norm_relu(batch_norm, x, name="bn" + idx, _tf32=tf32, **norm_kw)
+  h = batch_norm(x, name="bn" + idx, **norm_kw)
+  return ops.layer_norm(h, norm_kw["is_training"], "ln" + idx, _relu=True, _tf32=tf32)
+
+
+def residual_block(inputs, plan, batch_norm, z, y, is_training, use_sn, layer_norm=False):
   """norm-relu-conv, norm-relu-conv plus the plan's shortcut.  A generator block resamples in its FIRST convolution, a
-  discriminator block in its SECOND (reference resnet_ops.py:93-102).
+  discriminator block in its SECOND (reference resnet_ops.py:93-102).  `layer_norm` puts ln1 / ln2 behind bn1 / bn2
+  (the `D.layer_norm` binding).
 
   What the reference runs as separate TF ops is folded into the convolutions' epilogues where that is exact:
   * the residual add is done by the LAST convolution evaluated (conv2 for the 3x3-shortcut family, the 1x1 shortcut for
     BigGAN's) — `_residual`;
   * a down-sampling block pools ONCE: avgpool(a) + avgpool(b) == avgpool(a + b), so both branches stay at full
     resolution until their sum;
-  * without a normaliser between the two convolutions (every discriminator here) the second ReLU is conv1's epilogue;
+  * without a normaliser between the two convolutions (a discriminator without layer norm) the second ReLU is conv1's
+    epilogue;
   * every tensor whose only consumer is a tensor-core convolution is stored TF32-rounded (`_tf32`)."""
   if inputs.shape[-1] != plan.cin:
     if plan.shortcut == "conv3x3_first":
@@ -129,18 +140,18 @@ def residual_block(inputs, plan, batch_norm, z, y, is_training, use_sn):
   first = plan.scale if plan.generator_side else "none"
   second = "none" if plan.generator_side else plan.scale
   norm_kw = dict(z=z, y=y, is_training=is_training)
-  plain = ops.configured_norm(batch_norm) is None          # no normaliser: bn1 / bn2 are the identity
+  plain = ops.configured_norm(batch_norm) is None and not layer_norm     # no normaliser between the convolutions
   with V.variable_scope(plan.name):
     skip = None
     if plan.shortcut == "conv3x3_first":
       skip = _block_conv(inputs, plan, plan.cin, plan.cout, plan.scale, "conv_shortcut", 3, use_sn, pool=False)
     # (a block fed by the 3-channel image runs its first convolutions in the exact-fp32 streaming kernels: no rounding)
-    h = ops.norm_relu(batch_norm, inputs, name="bn1", _tf32=plan.cin > 4, **norm_kw)
+    h = _norm_relu(batch_norm, layer_norm, inputs, "1", plan.cin > 4, norm_kw)
     if plain and first != "down":
       h = _block_conv(h, plan, plan.cin, plan.cout, first, "conv1", 3, use_sn, _relu=True, _tf32=True)
     else:
       h = _block_conv(h, plan, plan.cin, plan.cout, first, "conv1", 3, use_sn)
-      h = ops.norm_relu(batch_norm, h, name="bn2", _tf32=True, **norm_kw)
+      h = _norm_relu(batch_norm, layer_norm, h, "2", True, norm_kw)
     if plan.shortcut == "conv3x3_first":
       h = _block_conv(h, plan, plan.cout, plan.cout, second, "conv2", 3, use_sn, pool=False, _residual=skip)
       return ops.observe(K.avgpool2(h) if plan.scale == "down" else h)

@@ -27,7 +27,8 @@ class ResNetBlock(object):
                             self._shortcut_kind())
 
   def apply(self, inputs, z, y, is_training):
-    return netdef.residual_block(inputs, self.plan(), self.batch_norm, z, y, is_training, self._spectral_norm)
+    return netdef.residual_block(inputs, self.plan(), self.batch_norm, z, y, is_training, self._spectral_norm,
+                                 layer_norm=self._layer_norm)
 
   __call__ = apply
 

@@ -461,6 +461,284 @@ inline bool v4_ok(const void* a, const void* b, const void* c, const void* d, co
            reinterpret_cast<uintptr_t>(d) | reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(f)) & 15) == 0;
 }
 
+// ---- layer norm (arch_ops.py:448-450, tf.contrib.layers.layer_norm with begin_norm_axis=1, begin_params_axis=-1) ----
+// Sample i of x is the contiguous span [i*span, (i+1)*span), span = h*w*c; its moments run over the whole span, gamma and
+// beta are per channel (c = element index mod C).  stats[2i] = mean, stats[2i+1] = r = rsqrt(var + eps).  The per-sample
+// reductions split each span over several CTAs (so that a batch of 64 still fills the GPU), accumulate in float64 and
+// merge the CTA partials in chunk order in the last CTA of each sample (ticket counter, reset by that CTA): deterministic,
+// one launch, no atomics on values.
+
+constexpr int LN_THREADS = 256;
+
+struct LnMomentsF {      // shifted by the sample's first element, so the float64 second moment does not cancel
+  const float* x;
+  __device__ __forceinline__ void operator()(int i, long long span, long long j, int, double* v) const {
+    const double d = (double)x[i * span + j] - (double)x[i * span];
+    v[0] = d;
+    v[1] = d * d;
+  }
+};
+
+struct LnBwdSumsF {      // a = gamma*g: sum a, sum a*xhat
+  const float *g, *x, *stats, *gamma;
+  __device__ __forceinline__ void operator()(int i, long long span, long long j, int c, double* v) const {
+    const float xh = (x[i * span + j] - stats[2 * i]) * stats[2 * i + 1];
+    const float a = gamma[c] * g[i * span + j];
+    v[0] = a;
+    v[1] = (double)a * xh;
+  }
+};
+
+struct LnBwdBwdSumsF {   // sum a, sum a*xhat, sum w, sum w*xhat, sum w*a
+  const float *w, *g, *x, *stats, *gamma;
+  __device__ __forceinline__ void operator()(int i, long long span, long long j, int c, double* v) const {
+    const long long e = i * span + j;
+    const float xh = (x[e] - stats[2 * i]) * stats[2 * i + 1];
+    const float a = gamma[c] * g[e], wv = w[e];
+    v[0] = a;
+    v[1] = (double)a * xh;
+    v[2] = wv;
+    v[3] = (double)wv * xh;
+    v[4] = (double)wv * a;
+  }
+};
+
+// grid (chunks, n).  MOMENTS: NV = 2 shifted sums, merged over chunks with Chan et al.'s pairwise update, output
+// stats[2i], stats[2i+1]; otherwise out[i*NV + v] = (sum over the span) / span.
+template <class F, int NV, bool MOMENTS>
+__global__ void __launch_bounds__(LN_THREADS) ln_sample_reduce_kernel(F f, long long span, int C, long long per_chunk,
+                                                                      double* __restrict__ partial, unsigned* counters,
+                                                                      float* out, float eps) {
+  __shared__ double sh[LN_THREADS / 32][NV];
+  __shared__ unsigned s_ticket;
+  const int i = blockIdx.y, k = blockIdx.x, chunks = gridDim.x;
+  const long long j0 = (long long)k * per_chunk, j1 = min(span, j0 + per_chunk);
+  double acc[NV];
+#pragma unroll
+  for (int v = 0; v < NV; ++v) acc[v] = 0.0;
+  long long j = j0 + threadIdx.x;
+  int c = (int)(j % C);
+  const int step = LN_THREADS % C;
+#pragma unroll 4
+  for (; j < j1; j += LN_THREADS) {
+    double v[NV];
+    f(i, span, j, c, v);
+#pragma unroll
+    for (int q = 0; q < NV; ++q) acc[q] += v[q];
+    c += step;
+    if (c >= C) c -= C;
+  }
+#pragma unroll
+  for (int v = 0; v < NV; ++v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[v] += __shfl_xor_sync(0xffffffffu, acc[v], o);
+  }
+  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+    for (int v = 0; v < NV; ++v) sh[threadIdx.x >> 5][v] = acc[v];
+  __syncthreads();
+  if (threadIdx.x < NV) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < LN_THREADS / 32; ++w) s += sh[w][threadIdx.x];
+    partial[((long long)i * chunks + k) * NV + threadIdx.x] = s;
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_ticket = atomicAdd(&counters[i], 1u);
+  __syncthreads();
+  if (s_ticket != (unsigned)(chunks - 1)) return;
+  __threadfence();
+  if (threadIdx.x != 0) return;
+  const double* p = partial + (long long)i * chunks * NV;
+  if constexpr (MOMENTS) {
+    double n = 0.0, mean = 0.0, m2 = 0.0;          // of the shifted values
+    for (int q = 0; q < chunks; ++q) {
+      const double nb = (double)(min(span, (long long)(q + 1) * per_chunk) - (long long)q * per_chunk);
+      const double s = __ldcg(p + 2 * q), ss = __ldcg(p + 2 * q + 1);
+      const double mb = s / nb, m2b = fmax(ss - s * mb, 0.0);
+      const double tot = n + nb, delta = mb - mean;
+      mean += delta * nb / tot;
+      m2 += m2b + delta * delta * n * nb / tot;
+      n = tot;
+    }
+    out[2 * i] = (float)(mean + (double)f.x[(long long)i * span]);
+    out[2 * i + 1] = (float)(1.0 / sqrt(m2 / n + (double)eps));
+  } else {
+    for (int v = 0; v < NV; ++v) {
+      double s = 0.0;
+      for (int q = 0; q < chunks; ++q) s += __ldcg(p + q * NV + v);
+      out[(long long)i * NV + v] = (float)(s / (double)span);
+    }
+  }
+  counters[i] = 0u;
+}
+
+template <class F, int NV, bool MOMENTS>
+int ln_sample_reduce(cgan_ctx* ctx, F f, int n, long long span, int C, float* out, float eps) {
+  if (!ctx->counters) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: no ticket counters on this context%s", "layer norm");
+  long long want = (8ll * ctx->num_sms + n - 1) / n;
+  long long maxchunks = (span + 4 * LN_THREADS - 1) / (4 * LN_THREADS);
+  long long chunks = want < maxchunks ? want : maxchunks;
+  if (chunks < 1) chunks = 1;
+  long long per = (span + chunks - 1) / chunks;
+  chunks = (span + per - 1) / per;
+  void* ws = nullptr;
+  int rc = cgan_ws(ctx, (size_t)n * chunks * NV * sizeof(double), &ws);
+  if (rc) return rc;
+  ln_sample_reduce_kernel<F, NV, MOMENTS><<<dim3((unsigned)chunks, (unsigned)n), LN_THREADS, 0, ctx->stream>>>(
+      f, span, C, per, reinterpret_cast<double*>(ws), ctx->counters, out, eps);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+// W consecutive elements (W = 4: float4 loads / stores, needs C % 4 == 0 and 16-byte aligned tensors)
+template <int W>
+__device__ __forceinline__ void ldw(float* v, const float* p) {
+  if (W == 4) {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+  } else {
+    v[0] = *p;
+  }
+}
+template <int W>
+__device__ __forceinline__ void stw(float* p, const float* v) {
+  if (W == 4) *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  else *p = v[0];
+}
+
+// Elementwise passes: grid (blocks per sample, n); thread t of a sample handles elements j = (t + k*stride)*W.
+#define LN_EW_LOOP(W)                                                                  \
+  const int i = blockIdx.y;                                                            \
+  const long long stride = (long long)gridDim.x * blockDim.x * W;                      \
+  long long j = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * W;                \
+  int c = (int)(j % C);                                                                \
+  const int step = (int)(stride % C);                                                  \
+  for (; j < span; j += stride, c = (c + step >= C) ? c + step - C : c + step)
+
+template <int W>
+__global__ void ln_apply_kernel(float* __restrict__ y, const float* __restrict__ x, long long span, int C,
+                                const float* __restrict__ stats, const float* __restrict__ gamma,
+                                const float* __restrict__ beta, int act) {
+  const int relu = act & 1, rnd = (act & CGAN_ACT_ROUND_TF32) ? 1 : 0;
+  LN_EW_LOOP(W) {
+    const float mean = stats[2 * i], r = stats[2 * i + 1];
+    const long long e = (long long)i * span + j;
+    float v[W], gm[W], bt[W];
+    ldw<W>(v, x + e);
+    ldw<W>(gm, gamma + c);
+    ldw<W>(bt, beta + c);
+#pragma unroll
+    for (int q = 0; q < W; ++q) {
+      float o = (v[q] - mean) * (r * gm[q]) + bt[q];
+      if (relu) o = fmaxf(o, 0.f);
+      v[q] = rnd ? rna_tf32(o) : o;
+    }
+    stw<W>(y + e, v);
+  }
+}
+
+// dx = r * (a - mean(a) - xhat * mean(a*xhat)), a = gamma*g; sums[2i] = mean(a), sums[2i+1] = mean(a*xhat)
+template <int W>
+__global__ void ln_bwd_dx_kernel(float* __restrict__ dx, const float* __restrict__ g, const float* __restrict__ x,
+                                 long long span, int C, const float* __restrict__ stats, const float* __restrict__ gamma,
+                                 const float* __restrict__ sums, int rnd) {
+  LN_EW_LOOP(W) {
+    const float mean = stats[2 * i], r = stats[2 * i + 1], abar = sums[2 * i], m = sums[2 * i + 1];
+    const long long e = (long long)i * span + j;
+    float xv[W], gv[W], gm[W];
+    ldw<W>(xv, x + e);
+    ldw<W>(gv, g + e);
+    ldw<W>(gm, gamma + c);
+#pragma unroll
+    for (int q = 0; q < W; ++q) {
+      const float xh = (xv[q] - mean) * r;
+      const float o = r * (gm[q] * gv[q] - abar - xh * m);
+      xv[q] = rnd ? rna_tf32(o) : o;
+    }
+    stw<W>(dx + e, xv);
+  }
+}
+
+// vjp of (g, x, gamma) -> dx for the cotangent w, with P(w) = w - mean(w) - xhat*mean(w*xhat):
+//   d_g = gamma * r * P(w)
+//   d_x = -r^2 * (xhat * (A - 3 m q) + q * (a - abar) + m * w),  A = mean(w*a) - abar*wbar, m = mean(a*xhat), q = mean(w*xhat)
+// d_x is TF's: the variance of tf.nn.moments reads stop_gradient(mean), which drops the term -r^2 * m * (-wbar) of the
+// exact second derivative.  s5[5i..5i+4] = mean(a), mean(a*xhat), mean(w), mean(w*xhat), mean(w*a).
+template <int W>
+__global__ void ln_bwd_bwd_kernel(float* __restrict__ d_g, float* __restrict__ d_x, const float* __restrict__ w,
+                                  const float* __restrict__ g, const float* __restrict__ x, long long span, int C,
+                                  const float* __restrict__ stats, const float* __restrict__ gamma,
+                                  const float* __restrict__ s5, int rnd) {
+  LN_EW_LOOP(W) {
+    const float mean = stats[2 * i], r = stats[2 * i + 1];
+    const float abar = s5[5 * i], m = s5[5 * i + 1], wbar = s5[5 * i + 2], q = s5[5 * i + 3];
+    const float A = s5[5 * i + 4] - abar * wbar, r2 = r * r;
+    const long long e = (long long)i * span + j;
+    float xv[W], gv[W], wv[W], gm[W], og[W];
+    ldw<W>(xv, x + e);
+    ldw<W>(gv, g + e);
+    ldw<W>(wv, w + e);
+    ldw<W>(gm, gamma + c);
+#pragma unroll
+    for (int k = 0; k < W; ++k) {
+      const float xh = (xv[k] - mean) * r, a = gm[k] * gv[k];
+      og[k] = gm[k] * r * (wv[k] - wbar - xh * q);
+      const float o = -r2 * (xh * (A - 3.f * m * q) + q * (a - abar) + m * wv[k]);
+      xv[k] = rnd ? rna_tf32(o) : o;
+    }
+    if (d_g) stw<W>(d_g + e, og);
+    if (d_x) stw<W>(d_x + e, xv);
+  }
+}
+#undef LN_EW_LOOP
+
+// per-channel sums over all pixels (colreduce rows): dgamma = sum g*xhat, dbeta = sum g
+struct LnBwdF {
+  const float *g, *x, *stats;
+  long long hw;
+  __device__ __forceinline__ void operator()(long long r, int c, int C, long long, float* v) const {
+    const long long i = r / hw;
+    const float gv = g[r * C + c];
+    v[0] = gv * ((x[r * C + c] - stats[2 * i]) * stats[2 * i + 1]);
+    v[1] = gv;
+  }
+};
+// d_gamma of the double backward: sum g * r * P(w)
+struct LnBwdBwdGammaF {
+  const float *w, *g, *x, *stats, *s5;
+  long long hw;
+  __device__ __forceinline__ void operator()(long long r, int c, int C, long long, float* v) const {
+    const long long i = r / hw;
+    const float rr = stats[2 * i + 1], xh = (x[r * C + c] - stats[2 * i]) * rr;
+    v[0] = g[r * C + c] * rr * (w[r * C + c] - s5[5 * i + 2] - xh * s5[5 * i + 3]);
+  }
+};
+
+// grid for the elementwise passes: about 16 blocks per SM in all, at least one per sample
+inline dim3 ln_ew_grid(cgan_ctx* ctx, int n, long long span, int w) {
+  long long per = ((long long)ctx->num_sms * 16 + n - 1) / n;
+  long long need = (span / w + 255) / 256;
+  if (per > need) per = need;
+  if (per < 1) per = 1;
+  return dim3((unsigned)per, (unsigned)n);
+}
+
+// per-sample results that must outlive the reduction partials at the head of the workspace (colreduce reuses the head)
+int ln_tail(cgan_ctx* ctx, size_t floats, float** out) {
+  void* ws = nullptr;
+  const size_t need = (floats * sizeof(float) + 255) / 256 * 256;
+  int rc = cgan_ws(ctx, need + (size_t)64 * 1024 * 1024, &ws);
+  if (rc) return rc;
+  *out = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + ctx->ws_bytes - need);
+  return CGAN_OK;
+}
+
+#define LN_CHECK_SHAPE(ctx, n, span, c)                                                                              \
+  CGAN_REQUIRE(ctx, (n) > 0 && (n) <= 65535 && (c) > 0 && (span) > 0 && (span) % (c) == 0,                          \
+               "need 0 < n <= 65535 samples and a span that is a positive multiple of the channels")
+
 }  // namespace
 
 int cgan_colsum(cgan_ctx* ctx, float* out, const float* x, int groups, int64_t rows_per_group, int c) {
@@ -558,6 +836,81 @@ int cgan_bn_bwd_apply(cgan_ctx* ctx, float* dx, const float* dy, const float* x,
     bn_bwd_apply_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(dx, dy, x, total, c, rps, mean_var2c, eps, gamma, cond,
                                                                       sums2c, inv_count, round_tf32 ? 1 : 0);
   }
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_layer_norm_moments(cgan_ctx* ctx, float* stats2n, const float* x, int n, int64_t span, float eps) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, stats2n && x, "null pointer");
+  LN_CHECK_SHAPE(ctx, n, span, 1);
+  return ln_sample_reduce<LnMomentsF, 2, true>(ctx, LnMomentsF{x}, n, span, 1, stats2n, eps);
+}
+
+int cgan_layer_norm_apply(cgan_ctx* ctx, float* y, const float* x, int n, int64_t span, int c, const float* stats2n,
+                          const float* gamma, const float* beta, int act) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, y && x && stats2n && gamma && beta, "null pointer");
+  LN_CHECK_SHAPE(ctx, n, span, c);
+  CGAN_REQUIRE(ctx, (act & ~(1 | CGAN_ACT_ROUND_TF32)) == 0, "act must be 0 / 1 (ReLU), optionally | CGAN_ACT_ROUND_TF32");
+  if (c % 4 == 0 && v4_ok(y, x, gamma, beta, nullptr, nullptr))
+    ln_apply_kernel<4><<<ln_ew_grid(ctx, n, span, 4), 256, 0, ctx->stream>>>(y, x, span, c, stats2n, gamma, beta, act);
+  else
+    ln_apply_kernel<1><<<ln_ew_grid(ctx, n, span, 1), 256, 0, ctx->stream>>>(y, x, span, c, stats2n, gamma, beta, act);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_layer_norm_bwd(cgan_ctx* ctx, float* dx, float* dgamma, float* dbeta, const float* g, const float* x, int n,
+                        int64_t span, int c, const float* stats2n, const float* gamma, int round_tf32) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, g && x && stats2n && gamma, "null pointer");
+  LN_CHECK_SHAPE(ctx, n, span, c);
+  const long long hw = span / c;
+  float* sums = nullptr;
+  int rc = ln_tail(ctx, (size_t)2 * n, &sums);
+  if (rc) return rc;
+  if (dgamma || dbeta) {    // one read of (g, x) for both per-channel sums
+    rc = colreduce<LnBwdF, 2>(ctx, LnBwdF{g, x, stats2n, hw}, 1, (long long)n * hw, c, 1.0f, dgamma, dbeta);
+    if (rc) return rc;
+  }
+  if (!dx) return CGAN_OK;
+  rc = ln_sample_reduce<LnBwdSumsF, 2, false>(ctx, LnBwdSumsF{g, x, stats2n, gamma}, n, span, c, sums, 0.f);
+  if (rc) return rc;
+  if (c % 4 == 0 && v4_ok(dx, g, x, gamma, nullptr, nullptr))
+    ln_bwd_dx_kernel<4><<<ln_ew_grid(ctx, n, span, 4), 256, 0, ctx->stream>>>(dx, g, x, span, c, stats2n, gamma, sums,
+                                                                             round_tf32 ? 1 : 0);
+  else
+    ln_bwd_dx_kernel<1><<<ln_ew_grid(ctx, n, span, 1), 256, 0, ctx->stream>>>(dx, g, x, span, c, stats2n, gamma, sums,
+                                                                             round_tf32 ? 1 : 0);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_layer_norm_bwd_bwd(cgan_ctx* ctx, float* d_g, float* d_x, float* d_gamma, const float* w, const float* g,
+                            const float* x, int n, int64_t span, int c, const float* stats2n, const float* gamma,
+                            int round_tf32) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, w && g && x && stats2n && gamma, "null pointer");
+  LN_CHECK_SHAPE(ctx, n, span, c);
+  const long long hw = span / c;
+  float* s5 = nullptr;
+  int rc = ln_tail(ctx, (size_t)5 * n, &s5);
+  if (rc) return rc;
+  rc = ln_sample_reduce<LnBwdBwdSumsF, 5, false>(ctx, LnBwdBwdSumsF{w, g, x, stats2n, gamma}, n, span, c, s5, 0.f);
+  if (rc) return rc;
+  if (d_gamma) {
+    rc = colreduce<LnBwdBwdGammaF, 1>(ctx, LnBwdBwdGammaF{w, g, x, stats2n, s5, hw}, 1, (long long)n * hw, c, 1.0f, d_gamma,
+                                      nullptr);
+    if (rc) return rc;
+  }
+  if (!d_g && !d_x) return CGAN_OK;
+  if (c % 4 == 0 && v4_ok(d_g ? d_g : w, d_x ? d_x : w, w, g, x, gamma))
+    ln_bwd_bwd_kernel<4><<<ln_ew_grid(ctx, n, span, 4), 256, 0, ctx->stream>>>(d_g, d_x, w, g, x, span, c, stats2n, gamma, s5,
+                                                                              round_tf32 ? 1 : 0);
+  else
+    ln_bwd_bwd_kernel<1><<<ln_ew_grid(ctx, n, span, 1), 256, 0, ctx->stream>>>(d_g, d_x, w, g, x, span, c, stats2n, gamma, s5,
+                                                                              round_tf32 ? 1 : 0);
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }

@@ -2,9 +2,11 @@
 and records its vector-Jacobian product on the tape (tape.py).  The vjps of the ops a discriminator
 without normalisation is made of (convolutions, matmul, bias, (leaky) ReLU, pools, reshapes, adds) are
 written with the same taped ops, so second-order differentiation (WGAN-GP, gans/penalty_lib.py:59-82)
-works by construction for them.  The vjps of batch norm, softmax and spectral normalisation w.r.t. its
-weight launch raw kernels: differentiating THROUGH them (a gradient penalty on a discriminator with
-BN / attention) raises NotImplementedError instead of silently dropping the second-order terms.
+works by construction for them.  Layer norm's vjp is a taped backward op whose own vjp launches a double-
+backward kernel, so a layer-normalised critic trains under WGAN-GP as well (with TF's second-order convention,
+see layer_norm).  The vjps of batch norm, softmax and spectral normalisation w.r.t. its weight launch raw
+kernels: differentiating THROUGH them (a gradient penalty on a discriminator with BN / attention) raises
+NotImplementedError instead of silently dropping the second-order terms.
 
 These are the H100 stand-ins for the TF library calls the reference's ops library makes
 (arch_ops.py / resnet_ops.py / loss_lib.py / penalty_lib.py); file:line citations sit on each op.
@@ -1180,6 +1182,76 @@ def bn_infer(x, gamma, beta, eps, state, use_moving_averages, cond=False, relu_a
     # BigGAN's conditional gamma / beta depend on z through the hierarchical chunks; the moments are constants
     y.tan = bn_apply_jvp(tx, x, mv, eps, gamma, tg, tb, cond, y if relu_after else None)
   return y
+
+
+# ------------------------------------------------------------------------------------ layer norm
+
+LN_EPS = 1e-12      # tf.contrib.layers.layer_norm's float32 variance_epsilon
+
+
+def layer_norm(x, gamma, beta, relu_after=False, round_out=False):
+  """tf.contrib.layers.layer_norm(x) with begin_norm_axis=1, begin_params_axis=-1 (arch_ops.py:448-450): moments per
+  sample over everything but the batch axis, gamma / beta [C] per channel.  `relu_after` fuses the following tf.nn.relu,
+  `round_out` stores TF32-rounded values in math_mode 1 (the result only feeds a tensor-core convolution).
+
+  Its vjp is the taped op layer_norm_bwd, whose own vjp launches the double backward, so a gradient penalty
+  differentiates through it.  That second order is TF's graph, not the exact Hessian: tf.nn.moments reads
+  stop_gradient(mean) in the variance (include/cgan_b200.h, cgan_layer_norm_bwd_bwd).  No cross-replica collective: the
+  moments never leave a sample."""
+  _constant("layer_norm", x, gamma, beta)
+  n, c = x.shape[0], x.shape[-1]
+  span = x.numel // n
+  stats = empty(2 * n)
+  _call("layer_norm_moments", stats.ptr, x.ptr, n, span, LN_EPS)
+  y = empty(*x.shape)
+  rnd = bool(round_out) and tf32_on()
+  _call("layer_norm_apply", y.ptr, x.ptr, n, span, c, stats.ptr, gamma.ptr, beta.ptr,
+        (1 if relu_after else 0) | (_lib.ACT_ROUND_TF32 if rnd else 0))
+  y.tf32 = rnd
+  yv = DT(y.t) if relu_after else None
+  if relu_after:
+    y.relu_of = (yv, 0.0)
+    for fn in RELU_OBSERVERS:
+      fn(y.t > 0)
+  y_id = id(y)
+
+  def vjp(g, needs):
+    if relu_after and not _premasked(g, y_id):
+      g = act_bwd(g, yv, ACT_RELU)    # y>0 <=> pre-activation>0
+    if recording() and (needs[1] or needs[2]):
+      raise NotImplementedError("second-order differentiation through the gamma / beta gradients of layer_norm is not "
+                                "implemented (gradient penalties differentiate w.r.t. the input only)")
+    dgamma = _grad_out(gamma, c) if needs[1] else None
+    dbeta = _grad_out(beta, c) if needs[2] else None
+    return [layer_norm_bwd(g, x, gamma, stats, dgamma, dbeta, want_dx=needs[0]), dgamma, dbeta]
+  return attach("layer_norm", y, [x, gamma, beta], vjp)
+
+
+def layer_norm_bwd(g, x, gamma, stats, dgamma=None, dbeta=None, want_dx=True):
+  """dx of layer_norm for the cotangent g; dgamma / dbeta (when given) receive the parameter gradients from the same
+  launch.  Taped in (g, x, gamma): its vjp launches cgan_layer_norm_bwd_bwd."""
+  n, c = x.shape[0], x.shape[-1]
+  span = x.numel // n
+  dx = empty(*x.shape) if want_dx else None
+  rnd = want_dx and _grad_feeds_tc(x)
+  _call("layer_norm_bwd", None if dx is None else dx.ptr, None if dgamma is None else dgamma.ptr,
+        None if dbeta is None else dbeta.ptr, g.ptr, x.ptr, n, span, c, stats.ptr, gamma.ptr, int(rnd))
+  if dx is None:
+    return None
+  dx.tf32 = rnd
+
+  def vjp(w, needs):
+    _no_second_order("the layer-norm double backward")
+    d_g = empty(*g.shape) if needs[0] else None
+    d_x = empty(*x.shape) if needs[1] else None
+    d_gamma = _grad_out(gamma, c) if needs[2] else None
+    rnd_x = needs[1] and _grad_feeds_tc(x)
+    _call("layer_norm_bwd_bwd", None if d_g is None else d_g.ptr, None if d_x is None else d_x.ptr,
+          None if d_gamma is None else d_gamma.ptr, w.ptr, g.ptr, x.ptr, n, span, c, stats.ptr, gamma.ptr, int(rnd_x))
+    if d_x is not None:
+      d_x.tf32 = rnd_x
+    return [d_g, d_x, d_gamma]
+  return attach("layer_norm_bwd", dx, [g, x, gamma], vjp)
 
 
 # ------------------------------------------------------------------------------------ spectral norm

@@ -192,6 +192,28 @@ int cgan_bn_bwd_apply(cgan_ctx*, float* dx, const float* dy, const float* x, int
                       const float* mean_var2c, float eps, const float* gamma, int cond, const float* sums2c,
                       float inv_count, int round_tf32);
 
+/* ---- layer norm (arch_ops.py:448-450: tf.contrib.layers.layer_norm, begin_norm_axis=1, begin_params_axis=-1) -------
+ * x is [n, span] with span = h*w*c (NHWC samples): the moments of sample i run over its whole span, gamma and beta are
+ * [c].  stats2n[2i] = mean, stats2n[2i+1] = r = rsqrt(var + eps) (contrib's float32 eps is 1e-12).  Each span is split over
+ * several CTAs; their float64 partials are merged in a fixed order (Chan et al.'s pairwise update), so results are
+ * deterministic.  Workspace through the context; no host synchronisation (capturable). */
+int cgan_layer_norm_moments(cgan_ctx*, float* stats2n, const float* x, int n, int64_t span, float eps);
+/* y = (x - mean) * (r * gamma) + beta; act: 0 none, 1 ReLU, optionally | CGAN_ACT_ROUND_TF32 */
+int cgan_layer_norm_apply(cgan_ctx*, float* y, const float* x, int n, int64_t span, int c, const float* stats2n,
+                          const float* gamma, const float* beta, int act);
+/* backward for the cotangent g on y: dx = r * (a - mean(a) - xhat * mean(a*xhat)) with a = gamma*g, xhat = (x - mean)*r,
+ * means per sample; dgamma = sum g*xhat, dbeta = sum g over all pixels.  dx, dgamma, dbeta nullable; round_tf32: store
+ * dx rounded to the nearest TF32 value. */
+int cgan_layer_norm_bwd(cgan_ctx*, float* dx, float* dgamma, float* dbeta, const float* g, const float* x, int n,
+                        int64_t span, int c, const float* stats2n, const float* gamma, int round_tf32);
+/* double backward: the vjp of (g, x, gamma) -> dx above for the cotangent w on dx.  With P(w) = w - mean(w) -
+ * xhat*mean(w*xhat): d_g = gamma * r * P(w), d_gamma = sum over pixels of g * r * P(w), and d_x is the vjp of TF's graph,
+ * whose variance reads stop_gradient(mean): the exact d_x minus r^2 * mean(a*xhat) * mean(w) per sample.  Outputs
+ * nullable; round_tf32 applies to d_x. */
+int cgan_layer_norm_bwd_bwd(cgan_ctx*, float* d_g, float* d_x, float* d_gamma, const float* w, const float* g,
+                            const float* x, int n, int64_t span, int c, const float* stats2n, const float* gamma,
+                            int round_tf32);
+
 /* ---- spectral norm (arch_ops.py:453-535) -------------------------------------------------- */
 /* One power iteration on w[rows,cols]; left=1: u[rows], v[cols] (arch_ops.py:505-509,525); left=0: u[cols], v[rows]
  * (:511-513,527).  u is updated in place (:516); v and sigma are outputs; wbar = w / sigma (nullable). */
