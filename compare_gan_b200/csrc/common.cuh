@@ -90,6 +90,15 @@ __device__ __forceinline__ float rna_tf32(float x) {
   return __uint_as_float(u);
 }
 
+// element i of the counter-based uniform [0, 1) stream (cgan_random_uniform): SplitMix64 of (seed, i + 1), 24 mantissa bits
+__device__ __forceinline__ float splitmix_uniform(unsigned long long seed, unsigned long long i) {
+  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (i + 1ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  return (float)(z >> 40) * (1.0f / 16777216.0f);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

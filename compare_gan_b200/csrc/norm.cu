@@ -503,9 +503,12 @@ struct LnBwdBwdSumsF {   // sum a, sum a*xhat, sum w, sum w*xhat, sum w*a
   }
 };
 
-// grid (chunks, n).  MOMENTS: NV = 2 shifted sums, merged over chunks with Chan et al.'s pairwise update, output
-// stats[2i], stats[2i+1]; otherwise out[i*NV + v] = (sum over the span) / span.
-template <class F, int NV, bool MOMENTS>
+// What ln_sample_reduce_kernel writes per sample: the NV means, or (NV = 2 shifted sums, merged over chunks with Chan et
+// al.'s pairwise update) mean and rsqrt(var + eps), or mean and var.
+enum LnOut { LN_MEANS, LN_MEAN_RSTD, LN_MEAN_VAR };
+
+// grid (chunks, n).  LN_MEANS: out[i*NV + v] = (sum over the span) / span; otherwise out[2i], out[2i+1] as LnOut says.
+template <class F, int NV, LnOut OUT>
 __global__ void __launch_bounds__(LN_THREADS) ln_sample_reduce_kernel(F f, long long span, int C, long long per_chunk,
                                                                       double* __restrict__ partial, unsigned* counters,
                                                                       float* out, float eps) {
@@ -551,7 +554,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_sample_reduce_kernel(F f, long 
   __threadfence();
   if (threadIdx.x != 0) return;
   const double* p = partial + (long long)i * chunks * NV;
-  if constexpr (MOMENTS) {
+  if constexpr (OUT != LN_MEANS) {
     double n = 0.0, mean = 0.0, m2 = 0.0;          // of the shifted values
     for (int q = 0; q < chunks; ++q) {
       const double nb = (double)(min(span, (long long)(q + 1) * per_chunk) - (long long)q * per_chunk);
@@ -563,7 +566,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_sample_reduce_kernel(F f, long 
       n = tot;
     }
     out[2 * i] = (float)(mean + (double)f.x[(long long)i * span]);
-    out[2 * i + 1] = (float)(1.0 / sqrt(m2 / n + (double)eps));
+    out[2 * i + 1] = OUT == LN_MEAN_VAR ? (float)(m2 / n) : (float)(1.0 / sqrt(m2 / n + (double)eps));
   } else {
     for (int v = 0; v < NV; ++v) {
       double s = 0.0;
@@ -574,7 +577,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_sample_reduce_kernel(F f, long 
   counters[i] = 0u;
 }
 
-template <class F, int NV, bool MOMENTS>
+template <class F, int NV, LnOut OUT>
 int ln_sample_reduce(cgan_ctx* ctx, F f, int n, long long span, int C, float* out, float eps) {
   if (!ctx->counters) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: no ticket counters on this context%s", "layer norm");
   long long want = (8ll * ctx->num_sms + n - 1) / n;
@@ -586,7 +589,7 @@ int ln_sample_reduce(cgan_ctx* ctx, F f, int n, long long span, int C, float* ou
   void* ws = nullptr;
   int rc = cgan_ws(ctx, (size_t)n * chunks * NV * sizeof(double), &ws);
   if (rc) return rc;
-  ln_sample_reduce_kernel<F, NV, MOMENTS><<<dim3((unsigned)chunks, (unsigned)n), LN_THREADS, 0, ctx->stream>>>(
+  ln_sample_reduce_kernel<F, NV, OUT><<<dim3((unsigned)chunks, (unsigned)n), LN_THREADS, 0, ctx->stream>>>(
       f, span, C, per, reinterpret_cast<double*>(ws), ctx->counters, out, eps);
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
@@ -739,6 +742,111 @@ int ln_tail(cgan_ctx* ctx, size_t floats, float** out) {
   CGAN_REQUIRE(ctx, (n) > 0 && (n) <= 65535 && (c) > 0 && (span) > 0 && (span) % (c) == 0,                          \
                "need 0 < n <= 65535 samples and a span that is a positive multiple of the channels")
 
+// ---- DRAGAN perturbation (penalty_lib.py:46-50) ----------------------------------------------------------------------
+// clip(x + std * (u - 0.5), 0, 1) with every operation rounded on its own, as TF's graph evaluates it (no FMA)
+__device__ __forceinline__ float dragan_noisy(float x, float sd, float u) {
+  return fmaxf(fminf(__fadd_rn(x, __fmul_rn(sd, u - 0.5f)), 1.0f), 0.0f);
+}
+
+// moments[1] is the batch variance; element i draws u from the stream at offset step * n + i.  n4 > 0: float4 body.
+__global__ void dragan_perturb_kernel(float* __restrict__ y, const float* __restrict__ x, long long n, long long n4,
+                                      unsigned long long seed, const int32_t* __restrict__ step,
+                                      const float* __restrict__ moments, float* __restrict__ std_out) {
+  const float sd = __fsqrt_rn(moments[1]);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *std_out = sd;
+  const unsigned long long off = (unsigned long long)*step * (unsigned long long)n;
+  const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+  for (long long v = t0; v < n4; v += stride) {
+    const float4 a = reinterpret_cast<const float4*>(x)[v];
+    const unsigned long long e = off + 4ull * (unsigned long long)v;
+    reinterpret_cast<float4*>(y)[v] = make_float4(
+        dragan_noisy(a.x, sd, splitmix_uniform(seed, e)), dragan_noisy(a.y, sd, splitmix_uniform(seed, e + 1)),
+        dragan_noisy(a.z, sd, splitmix_uniform(seed, e + 2)), dragan_noisy(a.w, sd, splitmix_uniform(seed, e + 3)));
+  }
+  for (long long i = 4 * n4 + t0; i < n; i += stride)
+    y[i] = dragan_noisy(x[i], sd, splitmix_uniform(seed, off + (unsigned long long)i));
+}
+
+// ---- L2 penalty over the kernels of a packed parameter buffer (penalty_lib.py:98-102) --------------------------------
+// Segment s = (segs[2s], segs[2s+1]) = (offset, length) in floats.  L2_LANES blocks share a segment, lane l reading the
+// float4s l*256 + t, l*256 + t + L2_LANES*256, ...: the summation order depends on this constant and the table only.
+constexpr int L2_LANES = 64;
+constexpr int L2_THREADS = 256;
+
+__device__ __forceinline__ long long l2_vec4(const float* base, long long off, long long len) {
+  return ((reinterpret_cast<uintptr_t>(base + off) & 15) == 0) ? len / 4 : 0;
+}
+
+// out[0] = mean over segments of sum(w^2) / 2: float64 squares and sums, per-lane partials merged in lane order and the
+// segments in table order by the last block (ticket counter, reset by that block), rounded once to fp32
+__global__ void __launch_bounds__(L2_THREADS) l2_penalty_kernel(float* __restrict__ out, const float* __restrict__ p,
+                                                                const long long* __restrict__ segs, int nseg,
+                                                                double* __restrict__ partial, unsigned* counter) {
+  __shared__ double sh[L2_THREADS / 32];
+  __shared__ unsigned s_ticket;
+  const int s = blockIdx.y, lane = blockIdx.x;
+  const long long off = segs[2 * s], len = segs[2 * s + 1], len4 = l2_vec4(p, off, len);
+  const float* w = p + off;
+  double acc = 0.0;
+  for (long long v = (long long)lane * L2_THREADS + threadIdx.x; v < len4; v += (long long)L2_LANES * L2_THREADS) {
+    const float4 a = reinterpret_cast<const float4*>(w)[v];
+    acc += (double)a.x * a.x;
+    acc += (double)a.y * a.y;
+    acc += (double)a.z * a.z;
+    acc += (double)a.w * a.w;
+  }
+  for (long long j = 4 * len4 + (long long)lane * L2_THREADS + threadIdx.x; j < len; j += (long long)L2_LANES * L2_THREADS)
+    acc += (double)w[j] * w[j];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int q = 0; q < L2_THREADS / 32; ++q) b += sh[q];
+    partial[(long long)s * L2_LANES + lane] = b;
+    __threadfence();
+    s_ticket = atomicAdd(counter, 1u);
+  }
+  __syncthreads();
+  if (s_ticket != (unsigned)(nseg * L2_LANES - 1)) return;
+  __threadfence();
+  for (int t = threadIdx.x; t < nseg; t += L2_THREADS) {       // each segment's lanes in order, in place of lane 0
+    double ss = 0.0;
+    for (int q = 0; q < L2_LANES; ++q) ss += __ldcg(partial + (long long)t * L2_LANES + q);
+    partial[(long long)t * L2_LANES] = 0.5 * ss;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  double tot = 0.0;
+  for (int t = 0; t < nseg; ++t) tot += partial[(long long)t * L2_LANES];
+  out[0] = (float)(tot / nseg);
+  *counter = 0u;
+}
+
+// g[seg] += fp32(fp32(scale[0] * mul) * w[seg]) over the segments only
+__global__ void __launch_bounds__(L2_THREADS) l2_penalty_bwd_kernel(float* __restrict__ g, const float* __restrict__ p,
+                                                                    const long long* __restrict__ segs,
+                                                                    const float* __restrict__ scale, float mul) {
+  const int s = blockIdx.y, lane = blockIdx.x;
+  const long long off = segs[2 * s], len = segs[2 * s + 1];
+  const long long len4 = l2_vec4(p, off, len) > 0 && l2_vec4(g, off, len) > 0 ? len / 4 : 0;
+  const float c = __fmul_rn(scale[0], mul);
+  const float* w = p + off;
+  float* d = g + off;
+  for (long long v = (long long)lane * L2_THREADS + threadIdx.x; v < len4; v += (long long)L2_LANES * L2_THREADS) {
+    const float4 a = reinterpret_cast<const float4*>(w)[v];
+    float4 b = reinterpret_cast<float4*>(d)[v];
+    b.x = __fadd_rn(b.x, __fmul_rn(c, a.x));
+    b.y = __fadd_rn(b.y, __fmul_rn(c, a.y));
+    b.z = __fadd_rn(b.z, __fmul_rn(c, a.z));
+    b.w = __fadd_rn(b.w, __fmul_rn(c, a.w));
+    reinterpret_cast<float4*>(d)[v] = b;
+  }
+  for (long long j = 4 * len4 + (long long)lane * L2_THREADS + threadIdx.x; j < len; j += (long long)L2_LANES * L2_THREADS)
+    d[j] = __fadd_rn(d[j], __fmul_rn(c, w[j]));
+}
+
 }  // namespace
 
 int cgan_colsum(cgan_ctx* ctx, float* out, const float* x, int groups, int64_t rows_per_group, int c) {
@@ -844,7 +952,7 @@ int cgan_layer_norm_moments(cgan_ctx* ctx, float* stats2n, const float* x, int n
   if (!ctx) return CGAN_ERR_ARG;
   CGAN_REQUIRE(ctx, stats2n && x, "null pointer");
   LN_CHECK_SHAPE(ctx, n, span, 1);
-  return ln_sample_reduce<LnMomentsF, 2, true>(ctx, LnMomentsF{x}, n, span, 1, stats2n, eps);
+  return ln_sample_reduce<LnMomentsF, 2, LN_MEAN_RSTD>(ctx, LnMomentsF{x}, n, span, 1, stats2n, eps);
 }
 
 int cgan_layer_norm_apply(cgan_ctx* ctx, float* y, const float* x, int n, int64_t span, int c, const float* stats2n,
@@ -875,7 +983,7 @@ int cgan_layer_norm_bwd(cgan_ctx* ctx, float* dx, float* dgamma, float* dbeta, c
     if (rc) return rc;
   }
   if (!dx) return CGAN_OK;
-  rc = ln_sample_reduce<LnBwdSumsF, 2, false>(ctx, LnBwdSumsF{g, x, stats2n, gamma}, n, span, c, sums, 0.f);
+  rc = ln_sample_reduce<LnBwdSumsF, 2, LN_MEANS>(ctx, LnBwdSumsF{g, x, stats2n, gamma}, n, span, c, sums, 0.f);
   if (rc) return rc;
   if (c % 4 == 0 && v4_ok(dx, g, x, gamma, nullptr, nullptr))
     ln_bwd_dx_kernel<4><<<ln_ew_grid(ctx, n, span, 4), 256, 0, ctx->stream>>>(dx, g, x, span, c, stats2n, gamma, sums,
@@ -897,7 +1005,7 @@ int cgan_layer_norm_bwd_bwd(cgan_ctx* ctx, float* d_g, float* d_x, float* d_gamm
   float* s5 = nullptr;
   int rc = ln_tail(ctx, (size_t)5 * n, &s5);
   if (rc) return rc;
-  rc = ln_sample_reduce<LnBwdBwdSumsF, 5, false>(ctx, LnBwdBwdSumsF{w, g, x, stats2n, gamma}, n, span, c, s5, 0.f);
+  rc = ln_sample_reduce<LnBwdBwdSumsF, 5, LN_MEANS>(ctx, LnBwdBwdSumsF{w, g, x, stats2n, gamma}, n, span, c, s5, 0.f);
   if (rc) return rc;
   if (d_gamma) {
     rc = colreduce<LnBwdBwdGammaF, 1>(ctx, LnBwdBwdGammaF{w, g, x, stats2n, s5, hw}, 1, (long long)n * hw, c, 1.0f, d_gamma,
@@ -911,6 +1019,49 @@ int cgan_layer_norm_bwd_bwd(cgan_ctx* ctx, float* d_g, float* d_x, float* d_gamm
   else
     ln_bwd_bwd_kernel<1><<<ln_ew_grid(ctx, n, span, 1), 256, 0, ctx->stream>>>(d_g, d_x, w, g, x, span, c, stats2n, gamma, s5,
                                                                               round_tf32 ? 1 : 0);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_dragan_perturb(cgan_ctx* ctx, float* y, const float* x, int64_t n, uint64_t seed, const int32_t* step_dev,
+                        float* std_out) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, y && x && step_dev && std_out, "null pointer");
+  CGAN_REQUIRE(ctx, n > 0, "need a non-empty batch");
+  float* moments = nullptr;
+  int rc = ln_tail(ctx, 2, &moments);
+  if (rc) return rc;
+  // the layer-norm moments of one "sample" spanning the whole batch, its variance instead of rsqrt(var + eps)
+  rc = ln_sample_reduce<LnMomentsF, 2, LN_MEAN_VAR>(ctx, LnMomentsF{x}, 1, n, 1, moments, 0.f);
+  if (rc) return rc;
+  const long long n4 = (al16(x) && al16(y)) ? n / 4 : 0;
+  dragan_perturb_kernel<<<ew_grid(ctx, n4 > 0 ? n4 : n), 256, 0, ctx->stream>>>(y, x, n, n4, seed, step_dev, moments,
+                                                                                std_out);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_l2_penalty(cgan_ctx* ctx, float* out, const float* flat_param, const int64_t* segs_dev, int nseg) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, out && flat_param && segs_dev, "null pointer");
+  CGAN_REQUIRE(ctx, nseg > 0 && nseg <= 65535, "need 0 < nseg <= 65535 segments");
+  if (!ctx->counters) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: no ticket counters on this context%s", "l2 penalty");
+  void* ws = nullptr;
+  int rc = cgan_ws(ctx, (size_t)nseg * L2_LANES * sizeof(double), &ws);
+  if (rc) return rc;
+  l2_penalty_kernel<<<dim3(L2_LANES, (unsigned)nseg), L2_THREADS, 0, ctx->stream>>>(
+      out, flat_param, reinterpret_cast<const long long*>(segs_dev), nseg, reinterpret_cast<double*>(ws), ctx->counters);
+  CGAN_LAUNCHED(ctx);
+  return CGAN_OK;
+}
+
+int cgan_l2_penalty_bwd(cgan_ctx* ctx, float* flat_grad, const float* flat_param, const int64_t* segs_dev, int nseg,
+                        const float* scale_dev, float mul) {
+  if (!ctx) return CGAN_ERR_ARG;
+  CGAN_REQUIRE(ctx, flat_grad && flat_param && segs_dev && scale_dev, "null pointer");
+  CGAN_REQUIRE(ctx, nseg > 0 && nseg <= 65535, "need 0 < nseg <= 65535 segments");
+  l2_penalty_bwd_kernel<<<dim3(L2_LANES, (unsigned)nseg), L2_THREADS, 0, ctx->stream>>>(
+      flat_grad, flat_param, reinterpret_cast<const long long*>(segs_dev), scale_dev, mul);
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }

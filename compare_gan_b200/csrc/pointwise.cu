@@ -793,13 +793,7 @@ int cgan_conv_post_epilogue(cgan_ctx* ctx, float* y, int64_t rows, int c, int ld
 
 namespace {
 __global__ void random_uniform_kernel(float* __restrict__ out, long long n, unsigned long long seed, unsigned long long offset) {
-  EW_LOOP(i, n) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (offset + (unsigned long long)i + 1ull);     // SplitMix64
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    out[i] = (float)(z >> 40) * (1.0f / 16777216.0f);
-  }
+  EW_LOOP(i, n) out[i] = splitmix_uniform(seed, offset + (unsigned long long)i);
 }
 }  // namespace
 

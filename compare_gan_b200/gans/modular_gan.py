@@ -87,6 +87,7 @@ class ModularGAN(AbstractGAN):
     self.store = V.VariableStore(seed=parameters.get("seed", 0))
     self._graph = None
     self._built_batch = None
+    self.d_kernels = None            # K.KernelSegments of D's kernels when the bound penalty is l2_penalty
 
   # ---- architecture registry (reference :169-213) ---------------------------------------------
   @property
@@ -143,7 +144,7 @@ class ModularGAN(AbstractGAN):
     if for_discriminator:
       penalty_loss = penalty_lib.get_penalty_loss(
           x=images, x_fake=generated, y=y, is_training=is_training, discriminator=self.discriminator,
-          alpha=features.get("alpha"))
+          alpha=features.get("alpha"), step=self.d_opt.step, kernel_segments=self.d_kernels)
       self.penalty_loss = penalty_loss
       if penalty_loss.node is not None:
         self.d_loss = K.add(self.d_loss, K.affine(penalty_loss, self._lambda))
@@ -175,6 +176,8 @@ class ModularGAN(AbstractGAN):
     self.store.reset_to_init()          # graph construction runs no ops: undo BN/u_var side effects
     self.g_opt = _FlatAdam(self._g_optimizer_fn(self._g_lr), self.flat_g)
     self.d_opt = _FlatAdam(self._d_optimizer_fn(self._d_lr), self.flat_d)
+    if penalty_lib.bound_penalty() is penalty_lib.l2_penalty:
+      self.d_kernels = K.KernelSegments(self.flat_d, penalty_lib.l2_kernels(self.store.trainable_under("discriminator")))
     self.ema = None
     if self._g_use_ema:
       self.ema = tape.DT(self.flat_g["param"].t.clone())
@@ -203,6 +206,8 @@ class ModularGAN(AbstractGAN):
         K.fill_(view, 0.0)                      # unreachable variable: zero gradient (tf.gradients would return None)
       elif g.ptr != view.ptr:                   # accumulated from several uses, or produced by an op without a sink
         K.copy_(view, g)
+    if prefix == "discriminator" and self.d_kernels is not None:
+      self.d_kernels.add_pending_grads()        # the L2 penalty's term, identical on every replica: the mean keeps it
     world = tpu_ops.num_replicas()
     if world > 1:
       tpu_ops.cross_replica_sum_(flat["grad"])

@@ -103,7 +103,7 @@ class SSGAN(ModularGAN):
     if for_discriminator:
       penalty_loss = penalty_lib.get_penalty_loss(
           x=images, x_fake=generated, y=y, is_training=is_training, discriminator=self.discriminator,
-          alpha=features.get("alpha"))
+          alpha=features.get("alpha"), step=self.d_opt.step, kernel_segments=self.d_kernels)
       self.penalty_loss = penalty_loss
       if penalty_loss.node is not None:
         self.d_loss = K.add(self.d_loss, K.affine(penalty_loss, self._lambda))

@@ -1411,6 +1411,53 @@ def gp_penalty(g):
   return attach("gp_penalty", pen, [g], lambda gg, needs: [_scale_by(dg, gg)])
 
 
+def dragan_perturb(x, seed, step):
+  """DRAGAN's perturbed real batch (penalty_lib.py:47-50): clip(x + std * (U - 0.5), 0, 1) with std the square root of
+  the variance over all of x, U uniform [0, 1) from the counter-based stream at (seed, step * numel(x)); `step` is an
+  int32 device counter read by the kernel, so a replayed CUDA graph draws at the counter's current value.  Returns
+  (y, std): y a fresh leaf like interpolate's, std a one-element device tensor."""
+  _constant("dragan_perturb", x)
+  y, std = empty(*x.shape), empty(1)
+  _call("dragan_perturb", y.ptr, x.ptr, x.numel, int(seed), step.data_ptr(), std.ptr)
+  return y, std
+
+
+class KernelSegments(object):
+  """The kernels among the variables of a packed parameter buffer (variables.VariableStore.pack): their (offset, length)
+  table, uploaded once for cgan_l2_penalty / cgan_l2_penalty_bwd, and the gradients l2_penalty's vjp leaves for
+  add_pending_grads."""
+
+  def __init__(self, flat, kernels):
+    """kernels: OrderedDict name -> DT of the selected variables, all packed in `flat`."""
+    self.flat, self.kernels = flat, kernels
+    pairs = [flat["views"][name] for name in kernels]
+    self.table = torch.tensor(pairs, dtype=torch.int64, device=_RT["device"]).reshape(-1)
+    self.n = len(pairs)
+    self.pending = []
+
+  def add_pending_grads(self):
+    """Adds scale * w / n into the kernel slots of the flat gradient buffer for every incoming gradient `scale` that
+    l2_penalty's vjp received, one launch each; call it after the slots hold the rest of their gradient."""
+    for scale in self.pending:
+      _call("l2_penalty_bwd", self.flat["grad"].ptr, self.flat["param"].ptr, self.table.data_ptr(), self.n, scale.ptr,
+            1.0 / self.n)
+    self.pending = []
+
+
+def l2_penalty(segs):
+  """mean over the kernels of tf.nn.l2_loss(w) = sum(w^2) / 2 (penalty_lib.py:98-102), one launch over the packed
+  buffer.  Taped in the kernel variables, but its vjp returns no per-variable tensors: the gradient w / n goes straight
+  into the flat gradient buffer's kernel slots, in one launch, when the owner of the buffer calls
+  segs.add_pending_grads().  Its gradient needs no second order."""
+  out = empty(1)
+  _call("l2_penalty", out.ptr, segs.flat["param"].ptr, segs.table.data_ptr(), segs.n)
+
+  def vjp(g, needs):
+    segs.pending.append(g)
+    return [None] * segs.n
+  return attach("l2_penalty", out, list(segs.kernels.values()), vjp)
+
+
 def set_math_mode(mode):
   """0: exact fp32 SIMT contractions; 1: wgmma TF32 tensor-core convolutions where the shape allows
   (operands rounded to nearest TF32, fp32 accumulation)."""

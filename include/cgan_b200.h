@@ -214,6 +214,24 @@ int cgan_layer_norm_bwd_bwd(cgan_ctx*, float* d_g, float* d_x, float* d_gamma, c
                             const float* x, int n, int64_t span, int c, const float* stats2n, const float* gamma,
                             int round_tf32);
 
+/* ---- DRAGAN and L2 penalties (penalty_lib.py:33-57, 85-103) ------------------------------------------------------ */
+/* DRAGAN's perturbed real batch (penalty_lib.py:47-50): y = clip(x + std * (U - 0.5), 0, 1) over the n floats of x, with
+ * var the float64 variance of all n elements rounded once to fp32 (the layer-norm moments of one sample spanning the
+ * batch), std = sqrtf(var), and U[i] = cgan_random_uniform's element at (seed, offset = step * n + i), step read from the
+ * device counter step_dev (the discriminator's Adam step before its update).  Each operation rounds on its own.  std is
+ * also written to the device scalar std_out.  Two launches, no host synchronisation (capturable; replays draw at the
+ * counter's new value). */
+int cgan_dragan_perturb(cgan_ctx*, float* y, const float* x, int64_t n, uint64_t seed, const int32_t* step_dev,
+                        float* std_out);
+/* L2 penalty over the kernels of a packed parameter buffer (penalty_lib.py:98-102): segs_dev holds nseg (offset, length)
+ * pairs in floats; out[0] = mean over segments of sum(w^2) / 2, squared and summed in float64 in an order fixed by the
+ * table alone, rounded once to fp32.  One launch. */
+int cgan_l2_penalty(cgan_ctx*, float* out, const float* flat_param, const int64_t* segs_dev, int nseg);
+/* its gradient: flat_grad[j] += fp32(fp32(scale_dev[0] * mul) * flat_param[j]) for every j inside a segment; nothing
+ * else is touched.  One launch. */
+int cgan_l2_penalty_bwd(cgan_ctx*, float* flat_grad, const float* flat_param, const int64_t* segs_dev, int nseg,
+                        const float* scale_dev, float mul);
+
 /* ---- spectral norm (arch_ops.py:453-535) -------------------------------------------------- */
 /* One power iteration on w[rows,cols]; left=1: u[rows], v[cols] (arch_ops.py:505-509,525); left=0: u[cols], v[rows]
  * (:511-513,527).  u is updated in place (:516); v and sigma are outputs; wbar = w / sigma (nullable). */
