@@ -135,6 +135,11 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* ac
   }
 }
 
+// CTAs per SM the register allocation has to allow.  The register file is split among the SM's four schedulers: two
+// CTAs of nine warps put five warps on one of them, so each thread may hold at most 16384 / (5 x 32) -> 96 registers.
+// At 100 registers the 128-column tile ran one CTA per SM although its shared memory fits two.
+constexpr int tc_min_ctas(int bn, int mt) { return bn * mt <= 128 ? 2 : 1; }
+
 // round this warpgroup's `bytes` of a tile (float4 per thread and sweep) to nearest TF32 in place
 __device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, int nthreads) {
 #pragma unroll 4
@@ -146,7 +151,7 @@ __device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, i
 }
 
 template <int BN, int MT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, tc_min_ctas(BN, MT))
 conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve: [stages][MT x A 16KB][B BN*128B] | barriers
@@ -434,6 +439,29 @@ inline int tc_pick_bn_occupancy(int ncols_pad, long long tiles_m, int sms) {
   return pick;
 }
 
+// Column tile of the per-tap kernel.  A 256-wide tile holds 128 fp32 accumulators per consumer thread, so only one CTA
+// fits on an SM and the tensor cores idle through every epilogue store and pipeline fill.  Two 128-wide CTAs share an SM
+// and one's epilogue overlaps the other's main loop; that is worth more than the doubled activation bytes per MMA while
+// the K loop is short (on H100: the generator's 3x3 256->256 convolutions at 16x16 and 32x32, batch 256, 72 k-blocks,
+// run 15-20 % faster) but not once it is long (BigGAN-128's 768-column convolutions at 16x16, 216 k-blocks, 35 % slower).
+// So the tile is halved when there are at least TC_NARROW_WAVES waves of 256-wide CTAs (pixel tiles x column tiles x
+// phases) and at most TC_NARROW_MAX_KB k-blocks (taps of the longest phase x 32-channel chunks) per CTA.  The K order is
+// unchanged, so the result is bit-identical to the wide tile's.
+constexpr int TC_NARROW_WAVES = 2;
+constexpr int TC_NARROW_MAX_KB = 96;
+
+inline int tc_pick_bn_per_tap(int ncols_pad, long long tiles_m, const TcParams& p, int sms) {
+  const int bn = tc_pick_bn_occupancy(ncols_pad, tiles_m, sms);
+  int kb = 0;
+  for (int i = 0; i < p.nphases; ++i) {
+    const int k = (p.ph_tap0[i + 1] - p.ph_tap0[i]) * p.kchunks;
+    if (k > kb) kb = k;
+  }
+  if (bn == 256 && tiles_m * (ncols_pad / 256) * p.nphases >= (long long)TC_NARROW_WAVES * sms && kb <= TC_NARROW_MAX_KB)
+    return 128;
+  return bn;
+}
+
 
 // every output row of the launch starts at an even element offset and the column count is even: float2 epilogue
 inline int tc_vec2(const TcParams& p) {
@@ -468,6 +496,14 @@ bool make_weight_map(CUtensorMap* tm, float* wt, int kdim_pad, int ncols_pad, in
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// CTAs of `kernel` that fit on one SM at `smem` bytes of dynamic shared memory (CGAN_OPT_LAST_TC_CTAS_PER_SM)
+template <typename Kernel>
+int tc_ctas_per_sm(Kernel kernel, size_t smem) {
+  int blocks = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kernel, TC_THREADS, smem) != cudaSuccess) blocks = 0;
+  return blocks;
+}
+
 // halo: the halo kernel, reading the activation box through as.m[0]
 template <int BN, int MT>
 int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
@@ -477,12 +513,14 @@ int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& a
       CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_halo_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set[1] = true;
     }
+    ctx->last_tc_ctas_per_sm = tc_ctas_per_sm(conv_tc_halo_kernel<BN, MT>, smem);
     conv_tc_halo_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as.m[0], b, p);
   } else {
     if (!attr_set[0]) {
       CGAN_CUDA(ctx, cudaFuncSetAttribute(conv_tc_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set[0] = true;
     }
+    ctx->last_tc_ctas_per_sm = tc_ctas_per_sm(conv_tc_kernel<BN, MT>, smem);
     conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p);
   }
   CGAN_LAUNCHED(ctx);
@@ -545,7 +583,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   if (c.wimg_stride != 0 && p.bni != 1)
     return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: batched GEMM needs >= 128 rows per matrix%s", "cgan_conv_tc");
   const int ncols_pad = (c.ncols + 31) / 32 * 32;
-  p.bn = tc_pick_bn_occupancy(ncols_pad, (long long)p.tiles_w * p.tiles_h * tiles_n, ctx->num_sms);
+  p.bn = tc_pick_bn_per_tap(ncols_pad, (long long)p.tiles_w * p.tiles_h * tiles_n, p, ctx->num_sms);
   p.cout = c.ncols;
   p.s_n = c.s_n; p.s_h = c.s_h; p.s_w = c.s_w; p.base = c.base;
   p.out = c.out;
@@ -635,7 +673,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
     // not eligible after all: restore the standard geometry
     tc_geometry(n, gh, gw, &p.bw, &p.bh, &p.bni, &p.tiles_w, &p.tiles_h, &tiles_n);
     p.rows_used = p.bw * p.bh * p.bni;
-    p.bn = tc_pick_bn_occupancy(ncols_pad, (long long)p.tiles_w * p.tiles_h * tiles_n, ctx->num_sms);
+    p.bn = tc_pick_bn_per_tap(ncols_pad, (long long)p.tiles_w * p.tiles_h * tiles_n, p, ctx->num_sms);
     p.hg = p.hnv = 0;
   }
 
@@ -650,10 +688,10 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
 
   // Pixel tiles per CTA: with mt = 2 the weight tile is fetched once for 256 pixels, which cuts the L2->SM bytes per MMA
   // by a third; only when enough CTAs remain to fill the machine.  Up to ~110 KB of smem per CTA when mt x bn <= 128, so
-  // that two CTAs share an SM and one's epilogue overlaps the other's main loop.  That overlap is worth more than the
-  // bytes: on H100 a 128-column tile at mt = 1 (two CTAs per SM) runs the 3x3 128->128 conv at 32x32, batch 512, in
-  // 0.97 ms against 1.39 ms at mt = 2 (one CTA per SM, the register file holds one 256-column accumulator set).  So
-  // mt = 2 only where two such CTAs still share an SM: bn <= 64.
+  // that two CTAs share an SM (tc_min_ctas keeps the registers within that too) and one's epilogue overlaps the other's
+  // main loop.  That overlap is worth more than the bytes: on H100 the 3x3 128->128 conv at 32x32, batch 512, takes
+  // 0.74 ms at bn = 128, mt = 1 (two CTAs per SM) against 1.39 ms at mt = 2 (one CTA per SM).  So mt = 2 only where two
+  // such CTAs still share an SM: bn <= 64.
   const long long tiles_total = (long long)p.tiles_w * p.tiles_h * tiles_n;
   const int ncol_tiles = ncols_pad / p.bn;
   p.tiles_total = (int)tiles_total;
