@@ -15,6 +15,9 @@
 //   (operand rounding,) wgmma m64nBNk8 (K = 8 per instruction, fp32 accumulators in registers), epilogue straight from
 //   the accumulator fragments (+bias, residual, ReLU / mask, TF32 rounding -> global); warp 8 = TMA producer.
 //   Stages are released one k-block late (wgmma.wait_group 1), so the rounding of the next stage overlaps the MMAs.
+// * A residual or ReLU mask (tensors of the output's geometry, far larger than L2 in a training step) is not read by
+//   the epilogue from global memory: after its last k-block the producer goes on around the stage ring and TMA-loads the
+//   CTA's tile of it, one 32-column chunk per stage, while the consumers finish their MMAs.
 //
 // The same kernel serves forward and input-gradient convolutions (and the four sub-pixel phases of a
 // conv over a zero-inserted 2x upsampled input): the host supplies, per tap, the input offset and the weight
@@ -71,9 +74,11 @@ struct TcParams {
   int a_halo_bytes;                 // smem footprint of one tile's halo box (1024-aligned)
   int a_box_bytes;                  // bytes TMA writes per halo box
   int sa_stages, sb_stages;
+  int ep_smem;                      // 1: the residual or mask is prefetched into the stage ring (tile_epilogue_smem)
 };
 
-// up to four views of the input tensor (the sub-pixel phases of a 2x-upsampled gradient); plain convs use view 0
+// up to four views of the input tensor (the sub-pixel phases of a 2x-upsampled gradient); plain convs use view 0.  The
+// same holds views of the residual / mask, one per output phase.
 struct AMaps { CUtensorMap m[4]; };
 
 
@@ -135,6 +140,65 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* ac
   }
 }
 
+// The same epilogue for a launch whose residual or mask (never both) the producer prefetched into the stage ring: the
+// 32-column chunk cc of the tile arrives in the next slot as a [rows_used][32] box, 128B-swizzled, rows in the tile's
+// pixel order.  The bias of the CTA's columns sits in shared memory.  No global load is left between two stores, so the
+// stores of a tile issue back to back instead of each waiting for its own residual / mask load.  A slot that a later
+// chunk of this CTA needs is released as soon as both warpgroups have read it.  The arithmetic and its order are
+// tile_epilogue's.
+template <int BN>
+__device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const float* acc, int tile, int nb0, int wg, int warp,
+                                                 int lane, long long out_base, const uint8_t* smem, int stage_bytes,
+                                                 uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                                 int& chunk, int chunks, const float* s_bias) {
+  int ow0, oh0, n0;
+  tc_tile_origin(p, tile, ow0, oh0, n0);
+  const int c2 = (lane & 3) * 2;
+  bool ok[2];
+  long long roff[2];
+  int m[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
+    const int wi = m[h] % p.bw;
+    const int hi = (m[h] / p.bw) % p.bh;
+    const int ni = m[h] / (p.bw * p.bh);
+    ok[h] = m[h] < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.img_h && ow0 + wi < p.img_w;
+    roff[h] = out_base + (long long)(n0 + ni) * p.s_n + (long long)(oh0 + hi) * p.s_h + (long long)(ow0 + wi) * p.s_w + nb0;
+  }
+  const uint32_t bias_addr = smem_u32(s_bias);
+#pragma unroll
+  for (int cc = 0; cc < BN / 32; ++cc) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t e_addr = smem_u32(smem + stage * stage_bytes);
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = cc * 4 + jj, c = j * 8 + c2;
+      if (nb0 + c >= p.cout) continue;
+      const float2 b = p.bias ? lds64(bias_addr + c * 4) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!ok[h]) continue;
+        float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        const float2 e = lds64(e_addr + sw128_offset(m[h], jj * 8 + c2));
+        if (p.bias) { v.x += b.x; v.y += b.y; }
+        if (p.residual) { v.x += e.x; v.y += e.y; }
+        if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+        if (p.mask) { v.x = e.x > 0.f ? v.x : p.mask_leak * v.x; v.y = e.y > 0.f ? v.y : p.mask_leak * v.y; }
+        if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
+        *reinterpret_cast<float2*>(p.out + roff[h] + c) = v;
+      }
+    }
+    if (chunk + p.stages < chunks) {           // a later chunk of this CTA refills the slot
+      fence_proxy_async();
+      named_bar(1 + wg, 128);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+    }
+    ++chunk;
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+  }
+}
+
 // CTAs per SM the register allocation has to allow.  The register file is split among the SM's four schedulers: two
 // CTAs of nine warps put five warps on one of them, so each thread may hold at most 16384 / (5 x 32) -> 96 registers.
 // At 100 registers the 128-column tile ran one CTA per SM although its shared memory fits two.
@@ -152,15 +216,17 @@ __device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, i
 
 template <int BN, int MT>
 __global__ void __launch_bounds__(TC_THREADS, tc_min_ctas(BN, MT))
-conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p) {
+conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p,
+               const __grid_constant__ AMaps tm_e) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][MT x A 16KB][B BN*128B] | barriers
+  // carve: [stages][MT x A 16KB][B BN*128B] | barriers (256 B) | with ep_smem: the bias of the CTA's BN columns
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int b_bytes = BN * TC_BK * 4;
   constexpr int a_bytes = MT * TC_A_BYTES;
   constexpr int stage_bytes = a_bytes + b_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
+  float* s_bias = reinterpret_cast<float*>(smem + p.stages * stage_bytes + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tap0 = p.ph_tap0[blockIdx.z];
@@ -204,11 +270,28 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
         tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
+      if (p.ep_smem) {
+        // the residual / mask tiles, one 32-column chunk per slot of the ring: the first one lands while the consumers
+        // still run the last stages - 1 k-blocks.  Box rows past the grid are zero-filled and count in the bytes.
+        const CUtensorMap* em = &tm_e.m[blockIdx.z];
+        for (int t = 0; t < nt_here; ++t) {
+          int ow0, oh0, n0;
+          tc_tile_origin(p, tile0 + t, ow0, oh0, n0);
+          for (int cc = 0; cc < BN / 32; ++cc) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_expect_tx(&full_bar[stage], (uint32_t)(p.rows_used * TC_BK * 4));
+            tma_load_4d(smem + stage * stage_bytes, em, &full_bar[stage], nb0 + cc * 32, ow0, oh0, n0);
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
     }
   } else {
     // ===== consumer warpgroups =====
     const int wg = warp >> 2;
     const int q = threadIdx.x & 127;
+    if (p.ep_smem && p.bias)
+      for (int i = threadIdx.x; i < BN; i += 32 * TC_CWARPS) s_bias[i] = nb0 + i < p.cout ? p.bias[nb0 + i] : 0.f;
     float acc[MT][BN / 2];
 #pragma unroll
     for (int t = 0; t < MT; ++t)
@@ -249,11 +332,26 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
+    if (p.ep_smem) {
+      // the last k-block's stage goes back to the producer for the residual / mask chunks
+      if (prev >= 0 && q == 0) mbar_arrive(&empty_bar[prev]);
+      named_bar(3, 32 * TC_CWARPS);              // s_bias is written
+      int chunk = 0;
 #pragma unroll
-    for (int t = 0; t < MT; ++t) {
+      for (int t = 0; t < MT; ++t) {
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
-      if (t < nt_here) tile_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z]);
+        for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+        if (t < nt_here)
+          tile_epilogue_smem<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z], smem, stage_bytes,
+                                 full_bar, empty_bar, stage, phase, chunk, nt_here * (BN / 32), s_bias);
+      }
+    } else {
+#pragma unroll
+      for (int t = 0; t < MT; ++t) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
+        if (t < nt_here) tile_epilogue<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z]);
+      }
     }
   }
 }
@@ -470,6 +568,17 @@ inline int tc_vec2(const TcParams& p) {
   return (odd & 1) ? 0 : 1;
 }
 
+// The per-tap kernel prefetches the residual or the mask of a launch (tile_epilogue_smem) when it has one of them, not
+// both, and TMA can read it in the output's geometry: every phase's first element and the pixel strides 16-byte aligned,
+// and the float2 epilogue applies.  Any other launch reads its epilogue operands from global memory in tile_epilogue.
+inline bool tc_ep_smem_ok(const TcParams& p, const TcConv& c) {
+  const float* e = c.residual ? c.residual : c.mask;
+  if (!e || (c.residual && c.mask) || !p.vec2 || (reinterpret_cast<uintptr_t>(e) & 15)) return false;
+  long long a = p.s_n | p.s_h | p.s_w;
+  for (int i = 0; i < p.nphases; ++i) a |= p.ph_base[i];
+  return (a & 3) == 0;
+}
+
 // Weights -> TF32-rounded (nearest) K-major [taps_total][ncols_pad][kdim_pad] in the context workspace
 int prep_weights(cgan_ctx* ctx, const TcConv& c, int kdim_pad, int ncols_pad, float** out) {
   void* ws = nullptr;
@@ -506,7 +615,8 @@ int tc_ctas_per_sm(Kernel kernel, size_t smem) {
 
 // halo: the halo kernel, reading the activation box through as.m[0]
 template <int BN, int MT>
-int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
+int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p,
+                const AMaps& es) {
   static bool attr_set[2] = {false, false};
   if (halo) {
     if (!attr_set[1]) {
@@ -521,17 +631,19 @@ int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& a
       attr_set[0] = true;
     }
     ctx->last_tc_ctas_per_sm = tc_ctas_per_sm(conv_tc_kernel<BN, MT>, smem);
-    conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p);
+    conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p, es);
   }
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }
 
-// the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS
-int tc_launch(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p) {
-  ctx->last_tc_bn = p.bn; ctx->last_tc_mt = p.mt; ctx->last_tc_halo = halo ? 1 : 0;
+// the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS.  es: the
+// residual / mask views of a launch with ep_smem (unused otherwise)
+int tc_launch(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p,
+              const AMaps& es) {
+  ctx->last_tc_bn = p.bn; ctx->last_tc_mt = p.mt; ctx->last_tc_halo = halo ? 1 : 0; ctx->last_tc_ep_smem = p.ep_smem;
 #define TC_CASE(BN, MT) \
-  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p);
+  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p, es);
   TC_CASE(32, 1) TC_CASE(64, 1) TC_CASE(96, 1) TC_CASE(128, 1) TC_CASE(160, 1) TC_CASE(192, 1) TC_CASE(224, 1)
   TC_CASE(256, 1) TC_CASE(32, 2) TC_CASE(64, 2) TC_CASE(96, 2) TC_CASE(128, 2)
 #undef TC_CASE
@@ -667,7 +779,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
         p.vec2 = tc_vec2(p);
         size_t smem = (size_t)p.sa_stages * p.mt * p.a_halo_bytes + (size_t)p.sb_stages * b_bytes + 1024 + 512;
         dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles);
-        return tc_launch(ctx, true, grid, smem, tm_a, tm_b, p);
+        return tc_launch(ctx, true, grid, smem, tm_a, tm_b, p, tm_a);
       }
     }
     // not eligible after all: restore the standard geometry
@@ -705,7 +817,14 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   if (p.stages > TC_MAX_STAGES) p.stages = TC_MAX_STAGES;
   if (p.stages < 2) p.stages = 2;
   p.vec2 = tc_vec2(p);
-  size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/;
+  AMaps tm_e;
+  memset(&tm_e, 0, sizeof(tm_e));
+  p.ep_smem = tc_ep_smem_ok(p, c) ? 1 : 0;
+  for (int v = 0; p.ep_smem && v < p.nphases; ++v)
+    if (!make_act_map(&tm_e.m[v], (c.residual ? c.residual : c.mask) + p.ph_base[v], c.ncols, gw, gh, n, p.s_w, p.s_h,
+                      p.s_n, p.bw, p.bh, p.bni))
+      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(residual / mask) failed%s", "cgan_conv_tc");
+  size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/ + (p.ep_smem ? p.bn * 4 : 0) /*bias*/;
   dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles, (unsigned)p.nphases);
-  return tc_launch(ctx, false, grid, smem, tm_as, tm_b, p);
+  return tc_launch(ctx, false, grid, smem, tm_as, tm_b, p, tm_e);
 }

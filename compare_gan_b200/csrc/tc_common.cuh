@@ -79,6 +79,11 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ float2 lds64(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
+}
 __device__ __forceinline__ float lds32(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));

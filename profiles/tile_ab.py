@@ -9,6 +9,12 @@ reported (the filter gradient, which reports no geometry, is timed at the defaul
 events on the launching stream, 3 warm-ups + 10 timed launches per entry.  The card name, power limit and SM clock are
 read in the same call.
 
+Epilogue axis: the forward and the input gradient are timed bare ("fwd": a zero bias, which stays in L1; "dgrad": no
+epilogue) and with the epilogue operands the cycle gives them, read from HBM: "fwd+res" adds a bias and a residual of
+the output's shape (the last convolution of a residual block; not for the up-sampling convolutions, which never take
+one), "dgrad+mask" gates the result with a ReLU mask (leak 0) and stores it TF32-rounded (the fused ReLU backward).  The
+"gap" column is the epilogue row's time minus its bare row's time.
+
   python profiles/tile_ab.py --tree PARENT_TREE --tree . [--rounds 3] [--out tile_ab_out]
 """
 import argparse
@@ -95,13 +101,20 @@ def child(tree):
     x, w, bias = rand(b, h, h, cin), rand(k, k, cin, cout), K.zeros(cout)
     d = K.conv_desc(b, h, h, cin, cout, k, k, 1, up, "SAME")
     dy = rand(b, d.oh, d.ow, cout)
+    ep_bias = rand(cout)
+    res = None if up else rand(b, d.oh, d.ow, cout)
+    mask = (rand(b, h, h, cin), 0.0)
     taps = k * k / 4.0 if up else k * k        # useful taps per output pixel (the zeros of the upsampling are skipped)
     flop = 2.0 * b * d.oh * d.ow * taps * cin * cout
     with tape.no_record():
       for pre in (False, True):                 # operands rounded in the kernel / already TF32-rounded by their producer
         x.tf32 = dy.tf32 = K.tf32_on() if pre else False
         suffix = " pre" if pre else ""
-        for op, fn in (("fwd", lambda: K.conv2d(x, w, bias, upsample=up)), ("dgrad", lambda: K.conv2d_dgrad(d, dy, w))):
+        ops = [("fwd", lambda: K.conv2d(x, w, bias, upsample=up)), ("dgrad", lambda: K.conv2d_dgrad(d, dy, w))]
+        if res is not None:
+          ops.append(("fwd+res", lambda: K.conv2d(x, w, ep_bias, upsample=up, residual=res)))
+        ops.append(("dgrad+mask", lambda: K.conv2d_dgrad(d, dy, w, round_out=True, relu_mask=mask)))
+        for op, fn in ops:
           ms = timed(fn)
           rows.append({"shape": label, "op": op + suffix, "ms": ms, "gflop": flop / 1e9, "geometry": geometry(),
                        "digest": digest(fn())})
@@ -112,7 +125,7 @@ def child(tree):
           rows.append({"shape": label, "op": "wgrad%s" % suffix, "ms": ms, "gflop": flop / 1e9,
                        "geometry": "tc_mt %d" % mt, "digest": digest(fn())})
         lib.set_option(_lib.OPT_TC_MT, 2)
-    del x, w, dy
+    del x, w, dy, res, mask
     torch.cuda.empty_cache()
   print(json.dumps({"device": torch.cuda.get_device_name(0), "rows": rows}))
 
@@ -159,14 +172,25 @@ def main():
       entry[key + "_tf32_share"] = row["gflop"] / entry[key + "_ms"] / TF32_PEAK_TFLOPS      # GFLOP / ms = TFLOP/s
     entry["same_bits"] = len({run["rows"][i]["digest"] for t in args.tree for run in runs[t]}) == 1
     table.append(entry)
+  bare = {(e["shape"], e["op"]): e for e in table}
+  for e in table:
+    if "+" in e["op"]:
+      op, _, rest = e["op"].partition("+")
+      pre = " pre" if rest.endswith(" pre") else ""
+      b = bare[(e["shape"], op + pre)]
+      for key in "ab":
+        e[key + "_gap"] = e[key + "_ms"] - b[key + "_ms"]
   print("%s | %s -> %s" % (info["device"], info["card_before"], info["card_after"]))
   print("A = %s, B = %s, median of %d rounds" % (args.tree[0], args.tree[1], args.rounds))
-  print("%-34s %-10s %8s | %-28s %8s %6s | %-28s %8s %6s | %6s %s" % (
-      "shape", "op", "GFLOP", "A geometry", "A ms", "A pk%", "B geometry", "B ms", "B pk%", "B/A", "bits"))
+  print("%-34s %-15s %8s | %-28s %8s %6s %7s | %-28s %8s %6s %7s | %6s %s" % (
+      "shape", "op", "GFLOP", "A geometry", "A ms", "A pk%", "A gap", "B geometry", "B ms", "B pk%", "B gap", "B/A",
+      "bits"))
+  gap = lambda e, key: "%7.3f" % e[key + "_gap"] if key + "_gap" in e else "%7s" % "-"
   for e in table:
-    print("%-34s %-10s %8.1f | %-28s %8.3f %5.1f%% | %-28s %8.3f %5.1f%% | %6.3f %s" % (
-        e["shape"], e["op"], e["gflop"], e["a_geometry"], e["a_ms"], 100 * e["a_tf32_share"], e["b_geometry"], e["b_ms"],
-        100 * e["b_tf32_share"], e["b_ms"] / e["a_ms"], "same" if e["same_bits"] else "DIFFER"))
+    print("%-34s %-15s %8.1f | %-28s %8.3f %5.1f%% %s | %-28s %8.3f %5.1f%% %s | %6.3f %s" % (
+        e["shape"], e["op"], e["gflop"], e["a_geometry"], e["a_ms"], 100 * e["a_tf32_share"], gap(e, "a"),
+        e["b_geometry"], e["b_ms"], 100 * e["b_tf32_share"], gap(e, "b"), e["b_ms"] / e["a_ms"],
+        "same" if e["same_bits"] else "DIFFER"))
   os.makedirs(args.out, exist_ok=True)
   with open(os.path.join(args.out, "tile_ab.json"), "w") as f:
     json.dump({"info": info, "rows": table}, f, indent=1)
