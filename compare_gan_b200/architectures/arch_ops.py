@@ -103,10 +103,11 @@ def _bn_state(c, use_moving_averages):
 @gin.configurable(whitelist=["decay", "epsilon", "use_cross_replica_mean", "use_moving_averages"])
 def standardize_batch(inputs, is_training, decay=0.999, epsilon=1e-3, data_format="NHWC",
                       use_moving_averages=True, use_cross_replica_mean=None,
-                      _gamma=None, _beta=None, _cond=False, _relu=False, _tf32=False):
+                      _gamma=None, _beta=None, _cond=False, _relu=False, _tf32=False, _gamma_beta=None):
   """Batch standardisation (reference arch_ops.py:194-319).  The private `_gamma/_beta` arguments let
-  batch_norm / conditional_batch_norm fuse their scale+offset (and a following ReLU) into the same kernel; `_tf32`
-  says that the result only feeds tensor-core contractions (it is then stored TF32-rounded in math_mode 1)."""
+  batch_norm / conditional_batch_norm fuse their scale+offset (and a following ReLU) into the same kernel
+  (`_gamma_beta`: self_modulated_batch_norm's [2N, C] scale and offset); `_tf32` says that the result only feeds
+  tensor-core contractions (it is then stored TF32-rounded in math_mode 1)."""
   if data_format not in {"NCHW", "NHWC"}:
     raise ValueError("Invalid data_format {}. Allowed: NCHW, NHWC.".format(data_format))
   if data_format != "NHWC":
@@ -118,12 +119,13 @@ def standardize_batch(inputs, is_training, decay=0.999, epsilon=1e-3, data_forma
     raise ValueError("Inputs has unsupported rank. Expected 2 or 4 but got %d" % rank)
   c = inputs.shape[-1]
   st = _bn_state(c, use_moving_averages)
+  extra = {} if _gamma_beta is None else {"gamma_beta": _gamma_beta}
   if is_training:
     return K.bn_train(inputs, _gamma, _beta, epsilon, st if use_moving_averages else None, decay, cond=_cond,
                       relu_after=_relu, allreduce=tpu_ops.cross_replica_sum_ if use_cross_replica_mean else None,
-                      world=tpu_ops.num_replicas() if use_cross_replica_mean else 1, round_out=_tf32)
+                      world=tpu_ops.num_replicas() if use_cross_replica_mean else 1, round_out=_tf32, **extra)
   return K.bn_infer(inputs, _gamma, _beta, epsilon, st, use_moving_averages, cond=_cond, relu_after=_relu,
-                    round_out=_tf32)
+                    round_out=_tf32, **extra)
 
 
 @gin.configurable(blacklist=["inputs"])
@@ -170,6 +172,43 @@ def conditional_batch_norm(inputs, y, is_training, use_sn, center=True, scale=Tr
                              _tf32=_tf32)
 
 
+@gin.configurable(whitelist=["num_hidden"])
+def self_modulated_batch_norm(inputs, z, is_training, use_sn, center=True, scale=True, name="batch_norm",
+                              num_hidden=32, _relu=False, _tf32=False):
+  """Self-modulated batch norm (reference arch_ops.py:370-420; Chen et al. 2019): gamma and beta are an MLP of z,
+  gamma = linear(h) with bias 1, beta = linear(h), h = relu(linear(z, num_hidden)) or z itself when num_hidden = 0.
+  The MLP is one kernel (kernels.self_modulation); its [2N, C] output feeds the BN apply as a conditional gamma / beta."""
+  if z is None:
+    raise ValueError("You must provide z for self modulation.")
+  if not (center and scale):
+    raise NotImplementedError("self_modulated_batch_norm without its scale or offset is not implemented")
+  with V.variable_scope(name):
+    c = inputs.shape[-1]
+    _bn_state_peek(c)
+    with V.variable_scope("sbn"):
+      wh = bh = None
+      if num_hidden > 0:
+        with V.variable_scope("hidden"):
+          wh, bh = _linear_params(z.shape[1], num_hidden, use_sn=use_sn)
+      width = num_hidden if num_hidden > 0 else z.shape[1]
+      with V.variable_scope("gamma"):
+        wg, bg = _linear_params(width, c, bias_start=1.0, use_sn=use_sn)
+      with V.variable_scope("beta"):
+        wb, bb = _linear_params(width, c, use_sn=use_sn)
+      gamma_beta = K.self_modulation(z, wh, bh, wg, bg, wb, bb)
+    return standardize_batch(inputs, is_training=is_training, _gamma_beta=gamma_beta, _cond=True, _relu=_relu,
+                             _tf32=_tf32)
+
+
+def _linear_params(input_size, output_size, bias_start=0.0, use_sn=False):
+  """(kernel, bias) of a `linear` layer in the current scope, created as linear creates them: kernel, its u_var under
+  use_sn, bias."""
+  kernel = V.get_variable("kernel", (input_size, output_size), weight_initializer(stddev=0.02))
+  if use_sn:
+    kernel = spectral_norm(kernel)
+  return kernel, V.get_variable("bias", (output_size,), constant_init(bias_start))
+
+
 def configured_norm(norm_fn):
   """The gin-configured normaliser behind a network's `batch_norm` method (None when it is the identity)."""
   net = getattr(norm_fn, "__self__", None)
@@ -181,7 +220,7 @@ def norm_relu(norm_fn, inputs, _tf32=False, **kwargs):
   """relu(norm_fn(inputs)): when the configured normaliser is one of the BN kernels above, the ReLU is fused into the
   BN-apply kernel (one pass over the activation instead of two); any other normaliser is followed by a plain ReLU.
   `_tf32`: the result only feeds tensor-core contractions (stored TF32-rounded in math_mode 1)."""
-  if configured_norm(norm_fn) in (batch_norm, conditional_batch_norm):
+  if configured_norm(norm_fn) in (batch_norm, conditional_batch_norm, self_modulated_batch_norm):
     return norm_fn(inputs, _relu=True, _tf32=_tf32, **kwargs)
   return K.relu(norm_fn(inputs, **kwargs), round_tf32=_tf32)
 

@@ -1088,14 +1088,26 @@ class BNState(object):
     self.accu_mean = self.accu_var = self.accu_counter = self.update_accus = None
 
 
+def _gamma_beta_halves(gb, c):
+  """Untaped [N, C] views of the gamma and beta halves of a [2N, C] self_modulation output."""
+  n = gb.shape[0] // 2
+  assert gb.shape == (2 * n, c)
+  return DT(gb.t[:n]), DT(gb.t[n:])
+
+
 def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_after=False, allreduce=None, world=1,
-             round_out=False):
+             round_out=False, gamma_beta=None):
   """Training-mode standardize_batch (+ gamma/beta) (arch_ops.py:194-319, 353-366, 435-444).
 
   gamma/beta: [C] DTs, or [N,C] when cond (conditional BN); either may be None.
+  gamma_beta: instead of gamma / beta under cond, one [2N, C] tensor holding both (self_modulation); one tape input,
+  whose gradient is one [2N, C] buffer.
   allreduce(stats_dt) sums a [2C] buffer over replicas (cross-replica moments, tpu_ops.py:94-125).
   """
-  _constant("bn_train", x, gamma, beta)
+  _constant("bn_train", x, gamma, beta, gamma_beta)
+  if gamma_beta is not None:
+    assert cond and gamma is None and beta is None
+    gamma, beta = _gamma_beta_halves(gamma_beta, x.shape[-1])
   c = x.shape[-1]
   rows = x.numel // c
   rps = rows // x.shape[0]
@@ -1128,11 +1140,16 @@ def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_afte
     if relu_after and not _premasked(g, y_id):
       g = act_bwd(g, yv, ACT_RELU)    # y>0 <=> pre-activation>0
     sums = empty(2 * c)
-    dgamma = dbeta = None
-    if gamma is not None and needs[1]:
-      dgamma = _grad_out(gamma, *gamma.shape)
-    if beta is not None and needs[2]:
-      dbeta = _grad_out(beta, *beta.shape)
+    dgamma = dbeta = dgb = None
+    if gamma_beta is not None:
+      if needs[1]:
+        dgb = empty(*gamma_beta.shape)
+        dgamma, dbeta = _gamma_beta_halves(dgb, c)
+    else:
+      if gamma is not None and needs[1]:
+        dgamma = _grad_out(gamma, *gamma.shape)
+      if beta is not None and needs[2]:
+        dbeta = _grad_out(beta, *beta.shape)
     with no_record():
       _call("bn_bwd_reduce", sums.ptr, None if dgamma is None else dgamma.ptr, None if dbeta is None else dbeta.ptr,
             g.ptr, x.ptr, rows, c, rps, mv.ptr, float(eps), None if gamma is None else gamma.ptr, int(cond))
@@ -1147,13 +1164,21 @@ def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_afte
         _call("bn_bwd_apply", dx.ptr, g.ptr, x.ptr, rows, c, rps, mv.ptr, float(eps),
               None if gamma is None else gamma.ptr, int(cond), sums.ptr, 1.0 / count, int(rnd_dx))
         dx.tf32 = rnd_dx
-    return [dx, dgamma, dbeta]
-  return attach("bn_train", y, [x, gamma, beta], vjp)
+    return [dx, dgb] if gamma_beta is not None else [dx, dgamma, dbeta]
+  return attach("bn_train", y, [x, gamma_beta] if gamma_beta is not None else [x, gamma, beta], vjp)
 
 
-def bn_infer(x, gamma, beta, eps, state, use_moving_averages, cond=False, relu_after=False, round_out=False):
-  """Inference-mode standardize_batch: moving averages (arch_ops.py:66-119) or accumulators (:122-191)."""
+def bn_infer(x, gamma, beta, eps, state, use_moving_averages, cond=False, relu_after=False, round_out=False,
+             gamma_beta=None):
+  """Inference-mode standardize_batch: moving averages (arch_ops.py:66-119) or accumulators (:122-191).  gamma_beta as
+  in bn_train."""
   c = x.shape[-1]
+  if gamma_beta is not None:
+    assert cond and gamma is None and beta is None
+    gamma, beta = _gamma_beta_halves(gamma_beta, c)
+    t_gb, _ = _tk(gamma_beta)
+    if t_gb is not None:
+      gamma.tan, beta.tan = _gamma_beta_halves(t_gb, c)
   rows = x.numel // c
   rps = rows // x.shape[0]
   if use_moving_averages:
@@ -1182,6 +1207,46 @@ def bn_infer(x, gamma, beta, eps, state, use_moving_averages, cond=False, relu_a
     # BigGAN's conditional gamma / beta depend on z through the hierarchical chunks; the moments are constants
     y.tan = bn_apply_jvp(tx, x, mv, eps, gamma, tg, tb, cond, y if relu_after else None)
   return y
+
+
+# ------------------------------------------------------------------------------------ self-modulation
+
+def self_modulation(z, wh, bh, wg, bg, wb, bb):
+  """The scale and offset MLP of self_modulated_batch_norm (arch_ops.py:370-420) in one launch (csrc/modulation.cu):
+  h = relu(z wh + bh) (h = z when wh is None: num_hidden = 0), gamma = h wg + bg, beta = h wb + bb, returned as one
+  [2N, C] tensor, gamma in rows 0..N-1 and beta in rows N..2N-1 (bn_train / bn_infer take it as gamma_beta).  The
+  hidden ReLU reports its mask to RELU_OBSERVERS like every other ReLU."""
+  n, zd = z.shape
+  hidden = 0 if wh is None else wh.shape[1]
+  c = wg.shape[1]
+  gb = empty(2 * n, c)
+  h = empty(n, hidden) if hidden else None
+  _call("self_modulation_fwd", gb.ptr, None if h is None else h.ptr, z.ptr, n, zd, hidden,
+        None if wh is None else wh.ptr, None if bh is None else bh.ptr, wg.ptr, bg.ptr, wb.ptr, bb.ptr, c)
+  if h is not None and RELU_OBSERVERS:
+    for fn in RELU_OBSERVERS:
+      fn(h.t > 0)
+  t, k = _tk(z)
+  if t is not None:
+    _constant("self_modulation", wh, bh, wg, bg, wb, bb)
+    gb.tan = empty(2 * n * k, c)
+    _call("self_modulation_jvp", gb.tan.ptr, t.ptr, None if h is None else h.ptr, None if wh is None else wh.ptr,
+          wg.ptr, wb.ptr, n, zd, hidden, c, k)
+
+  def vjp(g, needs):
+    _no_second_order("self_modulation")
+    dz = empty(n, zd) if needs[0] else None
+    dwh = _grad_out(wh, zd, hidden) if needs[1] else None
+    dbh = _grad_out(bh, hidden) if needs[2] else None
+    dwg = _grad_out(wg, *wg.shape) if needs[3] else None
+    dbg = _grad_out(bg, c) if needs[4] else None
+    dwb = _grad_out(wb, *wb.shape) if needs[5] else None
+    dbb = _grad_out(bb, c) if needs[6] else None
+    ptr = lambda d: None if d is None else d.ptr
+    _call("self_modulation_bwd", ptr(dwh), ptr(dbh), ptr(dwg), ptr(dbg), ptr(dwb), ptr(dbb), ptr(dz), g.ptr, ptr(h),
+          z.ptr, ptr(wh), wg.ptr, wb.ptr, n, zd, hidden, c)
+    return [dz, dwh, dbh, dwg, dbg, dwb, dbb]
+  return attach("self_modulation", gb, [z, wh, bh, wg, bg, wb, bb], vjp)
 
 
 # ------------------------------------------------------------------------------------ layer norm

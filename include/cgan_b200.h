@@ -199,6 +199,31 @@ int cgan_bn_bwd_apply(cgan_ctx*, float* dx, const float* dy, const float* x, int
                       const float* mean_var2c, float eps, const float* gamma, int cond, const float* sums2c,
                       float inv_count, int round_tf32);
 
+/* ---- self-modulated batch norm (arch_ops.py:370-420) -----------------------------------------------------------------
+ * The MLP that turns z [n, z_dim] into one layer's scale and offset: h = relu(z w_h + b_h) [n, hidden] (h = z when
+ * hidden = 0, the reference's num_hidden = 0), gamma = h w_gamma + b_gamma, beta = h w_beta + b_beta [n, c].  gb [2n, c]
+ * holds gamma in rows 0..n-1 and beta in rows n..2n-1: each half is the [samples, c] gamma / beta of
+ * cgan_bn_apply(cond = 1).  Weights are [in, out] as in linear.  K = hidden (or z_dim when hidden = 0) must be <= 256,
+ * n <= 12288.  Exact fp32 in both math modes; every output is summed in a fixed order without atomics, so reruns and
+ * graph replays are bit-identical.
+ * Forward: one launch; writes gb and (hidden > 0) h, the post-ReLU hidden state the backward reads. */
+int cgan_self_modulation_fwd(cgan_ctx*, float* gb, float* h, const float* z, int n, int z_dim, int hidden,
+                             const float* w_h, const float* b_h, const float* w_gamma, const float* b_gamma,
+                             const float* w_beta, const float* b_beta, int c);
+/* Backward for the cotangent dgb [2n, c]: dw_gamma = h^T dgamma, db_gamma = sum dgamma (beta alike); dh = (dgamma
+ * w_gamma^T + dbeta w_beta^T) * [h > 0], dw_h = z^T dh, db_h = sum dh, dz = dh w_h^T (dz = dh when hidden = 0).  Every
+ * output is nullable (dw_h / db_h need hidden > 0).  One launch for the wide layer, a second for dh's cross-CTA sum when
+ * dw_h, db_h or dz is asked for.  Workspace: per-CTA partials of dh, at most 64 MB. */
+int cgan_self_modulation_bwd(cgan_ctx*, float* dw_h, float* db_h, float* dw_gamma, float* db_gamma, float* dw_beta,
+                             float* db_beta, float* dz, const float* dgb, const float* h, const float* z,
+                             const float* w_h, const float* w_gamma, const float* w_beta, int n, int z_dim, int hidden,
+                             int c);
+/* Forward-mode tangent (biases and weights constant): t_z [n * k, z_dim] sample-major as cgan_act_jvp's batches,
+ * t_h = (t_z w_h) * [h[s] > 0] for the rows of sample s (t_h = t_z when hidden = 0), t_gb [2n * k, c] = t_h w_gamma in
+ * rows 0..nk-1 and t_h w_beta in rows nk..2nk-1: the t_gamma / t_beta halves cgan_bn_apply_jvp takes.  One launch. */
+int cgan_self_modulation_jvp(cgan_ctx*, float* t_gb, const float* t_z, const float* h, const float* w_h,
+                             const float* w_gamma, const float* w_beta, int n, int z_dim, int hidden, int c, int k);
+
 /* ---- layer norm (arch_ops.py:448-450: tf.contrib.layers.layer_norm, begin_norm_axis=1, begin_params_axis=-1) -------
  * x is [n, span] with span = h*w*c (NHWC samples): the moments of sample i run over its whole span, gamma and beta are
  * [c].  stats2n[2i] = mean, stats2n[2i+1] = r = rsqrt(var + eps) (contrib's float32 eps is 1e-12).  Each span is split over
