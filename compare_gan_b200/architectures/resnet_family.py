@@ -1,7 +1,8 @@
-"""The two "plain" ResNet pairs (CIFAR 32x32 and the five-block 128x128 one) share everything but their tables: a dense
-seed, residual blocks, BN-ReLU-conv3x3-sigmoid on the generator side; residual blocks, ReLU, spatial mean, dense logit
-(+ optional class projection) on the discriminator side.  The concrete modules (`resnet_cifar`, `resnet5`) only provide
-a `GeneratorPlan` / `DiscriminatorPlan`; this module runs them."""
+"""The "plain" ResNet pairs (CIFAR 32x32, the five-block 128x128 one, the 48x48 STL one and the 30-block 128x128 one)
+share everything but their tables: a dense seed, residual blocks, [BN-ReLU-]conv3x3-sigmoid on the generator side;
+[a colour convolution,] residual blocks, then ReLU and spatial mean or a plain flatten, dense logit (+ optional class
+projection) on the discriminator side.  The concrete modules (`resnet_cifar`, `resnet5`, `resnet_stl`, `resnet30`) only
+provide a `GeneratorPlan` / `DiscriminatorPlan`; this module runs them."""
 import collections
 
 from .. import kernels as K
@@ -12,12 +13,19 @@ from . import resnet_ops
 SEED = 4
 
 GeneratorPlan = collections.namedtuple(
-    "GeneratorPlan", "widths scales hierarchical_z embed_z embed_y spectral_norm_outside_blocks")
+    "GeneratorPlan", "widths scales hierarchical_z embed_z embed_y spectral_norm_outside_blocks seed names final_norm",
+    defaults=(SEED, None, True))
 # widths: seed width followed by each block's output width; scales: one of "up"/"none" per block;
-# spectral_norm_outside_blocks: whether the dense seed, the embeddings and the final conv follow G.spectral_norm
+# spectral_norm_outside_blocks: whether the dense seed, the embeddings and the final conv follow G.spectral_norm;
+# seed: side of the dense seed map; names: block names (None: B1, B2, ...); final_norm: BN-ReLU before final_conv
 
-DiscriminatorPlan = collections.namedtuple("DiscriminatorPlan", "first_block widths scales project_y")
-# first_block: index in the block names ("B0" or "B1"); widths: output width per block; scales: "down"/"none" per block
+DiscriminatorPlan = collections.namedtuple(
+    "DiscriminatorPlan", "first_block widths scales project_y names color_conv flatten power_of_two",
+    defaults=(None, None, False, True))
+# first_block: index in the block names ("B0" or "B1"); widths: output width per block; scales: "down"/"none" per block;
+# names: block names (None: B<first_block>, ...); color_conv: width of a 3x3 convolution (no spectral norm) in front of
+# the blocks, or None; flatten: the features are the last block's output flattened (NHWC order) rather than the spatial
+# mean of its ReLU; power_of_two: the input side must be a power of two
 
 
 class PlainResNetGenerator(resnet_ops.ResNetGenerator):
@@ -34,11 +42,15 @@ class PlainResNetGenerator(resnet_ops.ResNetGenerator):
       y = ops.linear(y, z.shape[1], scope="embed_y", use_sn=sn)
     z_seed, z_blocks, y_blocks = netdef.split_latent(z, y, len(plan.scales), plan.hierarchical_z)
     flow = netdef.Flow(self, z_seed, z=z, y=y, is_training=is_training)
-    flow.linear(SEED * SEED * plan.widths[0], "fc_noise", use_sn=sn).reshape(-1, SEED, SEED, plan.widths[0])
+    flow.linear(plan.seed * plan.seed * plan.widths[0], "fc_noise", use_sn=sn).reshape(-1, plan.seed, plan.seed,
+                                                                                        plan.widths[0])
     for i, scale in enumerate(plan.scales):
-      block = self._resnet_block("B%d" % (i + 1), plan.widths[i], plan.widths[i + 1], scale)
+      name = plan.names[i] if plan.names else "B%d" % (i + 1)
+      block = self._resnet_block(name, plan.widths[i], plan.widths[i + 1], scale)
       flow.x = block(flow.x, z=z_blocks[i], y=y_blocks[i], is_training=is_training)
-    flow.norm_relu("final_norm", tf32=True).conv(self._image_shape[2], 3, 1, "final_conv", use_sn=sn)
+    if plan.final_norm:
+      flow.norm_relu("final_norm", tf32=True)
+    flow.conv(self._image_shape[2], 3, 1, "final_conv", use_sn=sn)
     return K.sigmoid(flow.x)
 
 
@@ -48,16 +60,23 @@ class PlainResNetDiscriminator(resnet_ops.ResNetDiscriminator):
     raise NotImplementedError
 
   def apply(self, x, y, is_training):
-    resnet_ops.validate_image_inputs(x)
+    plan = self._plan(x.shape[-1])
+    resnet_ops.validate_image_inputs(x, validate_power2=plan.power_of_two)
     colors = x.shape[3]
     if colors not in (1, 3):
       raise ValueError("Number of color channels not supported: {}".format(colors))
-    plan = self._plan(colors)
     net, width = x, colors
+    if plan.color_conv:
+      net, width = ops.conv2d(x, plan.color_conv, 3, 3, 1, 1, name="color_conv"), plan.color_conv
     for i, (out_width, scale) in enumerate(zip(plan.widths, plan.scales)):
-      block = self._resnet_block("B%d" % (plan.first_block + i), width, out_width, scale)
+      name = plan.names[i] if plan.names else "B%d" % (plan.first_block + i)
+      block = self._resnet_block(name, width, out_width, scale)
       net, width = block(net, z=None, y=y, is_training=is_training), out_width
-    features = K.globalpool(K.relu(net), mean=True)
+    if plan.flatten:
+      features = K.reshape(net, net.shape[0], -1)
+      width = features.shape[1]
+    else:
+      features = K.globalpool(K.relu(net), mean=True)
     logit = ops.linear(features, 1, scope="disc_final_fc", use_sn=self._spectral_norm)
     if plan.project_y:
       if y is None:

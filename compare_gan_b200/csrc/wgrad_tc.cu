@@ -15,6 +15,9 @@
 // (deterministic), replacing TF's Conv2DBackpropFilter.
 // A conv over a zero-inserted 2x-upsampled input (resnet_ops.py:35-56) is handled through four strided TMA views of dY
 // (one per sub-pixel phase); every tap belongs to exactly one phase.
+// A grid whose width neither divides 32 nor is a multiple of it (the 48, 24, 12, 6 and 3 wide maps of a 48x48 network)
+// takes a box of at most 32 pixels that may hang over the grid's edge (`box_any`): TMA zero-fills the overrun, a zero dY
+// pixel adds nothing to dW, and the pixel rows the box leaves empty are zeroed once per CTA and never written again.
 #include "tc_common.cuh"
 
 namespace {
@@ -33,7 +36,7 @@ constexpr int WG_ACC_COLS = 256;         // mt x bn accumulator columns per CTA
 struct WgParams {
   int ntaps;
   int off_h[WG_MAX_TAPS], off_w[WG_MAX_TAPS], amap[WG_MAX_TAPS], bmap[WG_MAX_TAPS], wtap[WG_MAX_TAPS];
-  int bw, bh, bni, tiles_w, tiles_h;     // 32-pixel box geometry
+  int bw, bh, bni, tiles_w, tiles_h;     // box geometry: bw x bh x bni <= 32 pixels, tiles of the grid per box
   int kblocks, kb_per_split;
   int ci_tiles, co_tiles, bn;
   int cin, cout, taps_total;
@@ -41,6 +44,7 @@ struct WgParams {
   int mt;                                // (tap, ci-tile) units per CTA that share one dY tile (mt accumulator tiles)
   int round_a, round_b;                  // round the X / dY tiles to nearest TF32 (operand not pre-rounded)
   float* partial;                        // [split][taps_total][cin][cout]
+  int rows_used;                         // bw * bh * bni: pixel rows of a k-block the TMA box fills
 };
 
 struct BMaps { CUtensorMap m[4]; };
@@ -71,7 +75,8 @@ __device__ __forceinline__ void wg_transpose(uint32_t dst, uint32_t src, bool ro
   }
 }
 
-template <int BN, int MT>
+// PART: the box holds fewer than 32 pixels (box_any); box32's grids run the PART = false instantiations
+template <int BN, int MT, bool PART>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMaps tm_dy, const WgParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -105,6 +110,16 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if (PART) {
+    // a box of fewer than 32 pixels fills the same leading rows of every 4 KB box slot of the ring: zero the others once,
+    // so the transposition feeds zeros to the MMAs of the k-block's missing pixels
+    const int tail = (WG_P - p.rows_used) * 128;
+    const int words = p.stages * (stage_bytes / WG_BOX) * (tail / 16);
+    for (int i = threadIdx.x; i < words; i += WG_THREADS) {
+      const int slot = i / (tail / 16), off = i % (tail / 16);
+      sts128(smem_u32(smem + slot * WG_BOX + p.rows_used * 128) + off * 16, make_float4(0.f, 0.f, 0.f, 0.f));
+    }
+  }
   __syncthreads();
 
   if (warp == WG_CWARPS) {
@@ -123,7 +138,8 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem + stage * stage_bytes;
         uint8_t* sb = sa + a_bytes;
-        mbar_expect_tx(&full_bar[stage], (uint32_t)(nu * WG_A_BYTES + b_bytes));
+        mbar_expect_tx(&full_bar[stage], PART ? (uint32_t)((nu * 4 + BN / 32) * p.rows_used * 128)
+                                              : (uint32_t)(nu * WG_A_BYTES + b_bytes));
         for (int i = 0; i < nu; ++i) {
           const int u = u0 + i, utap = u / p.ci_tiles, ci0 = (u % p.ci_tiles) * 128;
           const CUtensorMap* ma = &tm_x.m[p.amap[utap]];
@@ -226,6 +242,27 @@ bool box32(int n, int h, int w, int* bw, int* bh, int* bni) {
   return true;
 }
 
+// A grid whose width neither divides 32 nor is a multiple of it: the box of at most 32 pixels, no larger than the grid in
+// any dimension, that needs the fewest k-blocks (ties: the wider box).  At batch 64: 48 -> 16x2, 24 -> 8x4, 12 -> 4x4 x 2
+// images, 6 -> 2x2 x 8, 3 -> 1x1 x 32, every MMA row a real pixel; at batch 4, 3 -> 3x3 x 3 (27 rows, the second image
+// tile half past the batch).  Every other width keeps box32's answer, or its refusal.
+bool box_any(int n, int h, int w, int* bw, int* bh, int* bni) {
+  if (n < 1 || h < 1 || w < 1 || 32 % w == 0 || w % 32 == 0) return false;
+  long long best = -1;
+  for (int b = w < 32 ? w : 32; b >= 1; --b)
+    for (int hh = 32 / b < h ? 32 / b : h; hh >= 1; --hh) {
+      const int ni = 32 / (b * hh) < n ? 32 / (b * hh) : n;
+      const long long kb = (long long)((w + b - 1) / b) * ((h + hh - 1) / hh) * ((n + ni - 1) / ni);
+      if (best < 0 || kb < best) { best = kb; *bw = b; *bh = hh; *bni = ni; }
+    }
+  return true;
+}
+
+// the box the kernel takes for an n x h x w grid; per-image launches (one k-block range per image) take box32's only
+bool wg_box(int n, int h, int w, bool per_image, int* bw, int* bh, int* bni) {
+  return box32(n, h, w, bw, bh, bni) || (!per_image && box_any(n, h, w, bw, bh, bni));
+}
+
 int pick_bn(int ncols) {
   if (ncols <= 256 && ncols % 4 == 0) return (ncols + 31) / 32 * 32;     // zero-padded tile, stores are masked
   if (ncols % 32) return 0;
@@ -247,22 +284,25 @@ size_t wg_smem(size_t stage_bytes, size_t budget, int* stages) {
   return (size_t)(s + 2) * stage_bytes + 1024 + 256;
 }
 
-template <int BN, int MT>
+template <int BN, int MT, bool PART>
 int wg_launch_t(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BMaps& tm_dy, const WgParams& p) {
   static bool attr_set = false;
   if (!attr_set) {
-    CGAN_CUDA(ctx, cudaFuncSetAttribute(wgrad_tc_kernel<BN, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CGAN_CUDA(ctx, cudaFuncSetAttribute(wgrad_tc_kernel<BN, MT, PART>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        227 * 1024));
     attr_set = true;
   }
-  wgrad_tc_kernel<BN, MT><<<grid, WG_THREADS, smem, ctx->stream>>>(tm_x, tm_dy, p);
+  wgrad_tc_kernel<BN, MT, PART><<<grid, WG_THREADS, smem, ctx->stream>>>(tm_x, tm_dy, p);
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }
 
-// one instantiation per (bn, mt): the accumulator fragment is sized at compile time
+// one instantiation per (bn, mt, partial box): the accumulator fragment is sized at compile time
 int wg_launch(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BMaps& tm_dy, const WgParams& p) {
-#define WG_CASE(BN, MT) \
-  if (p.bn == BN && p.mt == MT) return wg_launch_t<BN, MT>(ctx, grid, smem, tm_x, tm_dy, p);
+#define WG_CASE(BN, MT)                                                                                        \
+  if (p.bn == BN && p.mt == MT)                                                                                \
+    return p.rows_used < WG_P ? wg_launch_t<BN, MT, true>(ctx, grid, smem, tm_x, tm_dy, p)                    \
+                              : wg_launch_t<BN, MT, false>(ctx, grid, smem, tm_x, tm_dy, p);
   WG_CASE(32, 1) WG_CASE(64, 1) WG_CASE(96, 1) WG_CASE(128, 1) WG_CASE(160, 1) WG_CASE(192, 1) WG_CASE(224, 1)
   WG_CASE(256, 1) WG_CASE(32, 2) WG_CASE(64, 2) WG_CASE(96, 2) WG_CASE(128, 2)
 #undef WG_CASE
@@ -273,7 +313,7 @@ int wg_launch(cgan_ctx* ctx, dim3 grid, size_t smem, const BMaps& tm_x, const BM
 
 bool cgan_wgrad_tc_fits(const TcWgrad& g) {
   int bw, bh, bni;
-  return box32(g.dy.n, g.dy.h, g.dy.w, &bw, &bh, &bni) && (!g.per_image || (bni == 1 && g.dy.n <= 65535)) &&
+  return wg_box(g.dy.n, g.dy.h, g.dy.w, g.per_image, &bw, &bh, &bni) && (!g.per_image || (bni == 1 && g.dy.n <= 65535)) &&
          g.x.ch > 0 && g.x.ch % 32 == 0 &&            // ci tiles of 128, the last one zero-padded
          pick_bn(g.dy.ch) != 0 && g.taps.ntaps >= 1 && g.taps.ntaps <= WG_MAX_TAPS && al16(g.x.in) && al16(g.dy.in) &&
          al16(g.dw);
@@ -286,10 +326,11 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
   const int n = g.dy.n, gh = g.dy.h, gw = g.dy.w;      // the pixel grid
   p.round_a = g.x.tf32 ? 0 : 1;
   p.round_b = g.dy.tf32 ? 0 : 1;
-  box32(n, gh, gw, &p.bw, &p.bh, &p.bni);
-  p.tiles_w = gw / p.bw;
-  p.tiles_h = gh / p.bh;
-  p.kblocks = (int)((long long)n * gh * gw / WG_P);
+  wg_box(n, gh, gw, g.per_image, &p.bw, &p.bh, &p.bni);
+  p.rows_used = p.bw * p.bh * p.bni;
+  p.tiles_w = (gw + p.bw - 1) / p.bw;
+  p.tiles_h = (gh + p.bh - 1) / p.bh;
+  p.kblocks = (int)((long long)p.tiles_w * p.tiles_h * ((n + p.bni - 1) / p.bni));    // n * gh * gw / 32 for box32
   p.bn = pick_bn(g.dy.ch);
   p.ci_tiles = (g.x.ch + 127) / 128;
   p.co_tiles = (g.dy.ch + p.bn - 1) / p.bn;

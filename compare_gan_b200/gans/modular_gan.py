@@ -16,7 +16,8 @@ from .. import gin_lite as gin
 from .. import kernels as K
 from .. import tape
 from .. import variables as V
-from ..architectures import dcgan, resnet5, resnet_biggan, resnet_biggan_deep, resnet_cifar, sndcgan
+from ..architectures import (dcgan, resnet5, resnet30, resnet_biggan, resnet_biggan_deep, resnet_cifar, resnet_stl,
+                             sndcgan)
 from ..tpu import tpu_ops
 from . import consts, loss_lib, penalty_lib
 from .abstract_gan import AbstractGAN
@@ -99,7 +100,8 @@ class ModularGAN(AbstractGAN):
     if self._generator is None:
       module = {consts.RESNET5_ARCH: resnet5, consts.RESNET_BIGGAN_ARCH: resnet_biggan, consts.DCGAN_ARCH: dcgan,
                 consts.RESNET_BIGGAN_DEEP_ARCH: resnet_biggan_deep,
-                consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan}.get(self._architecture)
+                consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan, consts.RESNET30_ARCH: resnet30,
+                consts.RESNET_STL_ARCH: resnet_stl}.get(self._architecture)
       if module is None:
         raise NotImplementedError("Architecture {} not implemented.".format(self._architecture))
       self._generator = module.Generator(image_shape=self._dataset.image_shape)
@@ -110,7 +112,8 @@ class ModularGAN(AbstractGAN):
     if self._discriminator is None:
       module = {consts.RESNET5_ARCH: resnet5, consts.RESNET_BIGGAN_ARCH: resnet_biggan, consts.DCGAN_ARCH: dcgan,
                 consts.RESNET_BIGGAN_DEEP_ARCH: resnet_biggan_deep,
-                consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan}.get(self._architecture)
+                consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan, consts.RESNET30_ARCH: resnet30,
+                consts.RESNET_STL_ARCH: resnet_stl}.get(self._architecture)
       if module is None:
         raise NotImplementedError("Architecture {} not implemented.".format(self._architecture))
       self._discriminator = module.Discriminator()
