@@ -222,6 +222,7 @@ struct TcConv {
   float* out;
   long long s_n, s_h, s_w, base;
   long long ph_base[4];
+  int ph_h[4], ph_w[4];               // > 0: phase ph stores only rows < ph_h[ph], columns < ph_w[ph] (0: the whole grid)
   // epilogue: + bias[col] + residual, then ReLU or the (leaky-)ReLU backward gate out = mask > 0 ? v : mask_leak * v,
   // then TF32 rounding of the stored value
   const float* bias;
@@ -236,11 +237,16 @@ static inline void tc_out_dense(TcConv* c, float* y, int h, int w, int ld) {
   c->out = y; c->gh = h; c->gw = w;
   c->s_w = ld; c->s_h = (long long)w * ld; c->s_n = (long long)h * w * ld; c->base = 0;
 }
-// dense NHWC [.., H, W, c] written through its parity phases: an H/2 x W/2 grid, phase 2a + b at pixel (2i + a, 2j + b)
+// dense NHWC [.., H, W, c] written through its parity phases: a ceil(H/2) x ceil(W/2) grid, phase 2a + b at pixel
+// (2i + a, 2j + b).  Phase a holds the rows 2i + a < H, (H - a + 1) / 2 of them: for odd H the odd phases are one row
+// short, and the epilogue stores nothing past a phase's own extent.
 static inline void tc_out_phases(TcConv* c, float* y, int H, int W, int ch) {
-  c->out = y; c->gh = H / 2; c->gw = W / 2;
+  c->out = y; c->gh = (H + 1) / 2; c->gw = (W + 1) / 2;
   c->s_w = 2ll * ch; c->s_h = 2ll * W * ch; c->s_n = (long long)H * W * ch; c->base = 0;
-  for (int v = 0; v < 4; ++v) c->ph_base[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
+  for (int v = 0; v < 4; ++v) {
+    c->ph_base[v] = ((long long)(v >> 1) * W + (v & 1)) * ch;
+    c->ph_h[v] = (H - (v >> 1) + 1) / 2; c->ph_w[v] = (W - (v & 1) + 1) / 2;
+  }
 }
 // the whole epilogue of `ep` (null: none) and whether the activation operand is already TF32-rounded
 static inline void tc_set_epilogue(TcConv* c, const cgan_conv_epilogue* ep, bool in_tf32) {

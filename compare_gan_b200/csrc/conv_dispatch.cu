@@ -139,12 +139,21 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
   const bool ptr_ok = al16(dy) && al16(dx) && (!bias || al16(bias)) &&
                       (!ep || ((!ep->residual || al16(ep->residual)) && (!ep->mask || al16(ep->mask))));
   const bool geom = d->oh == (d->upsample ? 2 * d->h : d->h) && d->ow == (d->upsample ? 2 * d->w : d->w);
+  // stride 2 (also tf.nn.conv2d_transpose of SNDCGAN's generator, arch_ops.py:588-589): input pixel 2i+a only receives
+  // the taps with kh = a + pad_t (mod 2), from output row i + (a + pad_t - kh)/2 -> four input phases in one launch
+  // (grid.z = phase), each writing a strided quarter of dx.  An odd H has ceil(H/2) output rows, and the odd phases of dx
+  // are one row short of the even ones (tc_out_phases).
+  const bool s2_phases = ctx->math_mode == 1 && d->stride == 2 && !d->upsample && d->kh * d->kw <= 16 && d->h >= 2 &&
+                         d->w >= 2 && d->oh == (d->h + 1) / 2 && d->ow == (d->w + 1) / 2 && d->kh >= 2 && d->kw >= 2 &&
+                         cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cout, d->cin) && ptr_ok && d->cin % 4 == 0;
   if (ctx->tc_thin && ptr_ok && al16(w) && !(d->kh == 1 && d->kw == 1)) {
     if (cgan_thin_tc_cout_ok(ctx, d)) {          // dy has <= 4 channels (the generator's image conv)
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
       return cgan_thin_tc_dgrad_cout(ctx, d, dy, w, ep, dx);
     }
-    if (cgan_thin_tc_dgrad_cin_ok(ctx, d)) {     // dx has <= 4 channels (gradient w.r.t. the discriminator's input image)
+    // dx has <= 4 channels (gradient w.r.t. the discriminator's input image; the generator's stride-2 image layer).  A
+    // stride-2 shape the phase kernel takes stays there.
+    if (!s2_phases && cgan_thin_tc_dgrad_cin_ok(ctx, d)) {
       ctx->last_path = CGAN_PATH_TCGEN05_TF32;
       return cgan_thin_tc_dgrad_cin(ctx, d, dy, w, ep, dx);
     }
@@ -170,12 +179,7 @@ int cgan_conv2d_dgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* dy
     conv_taps(d, -1, TAP_VIEW, &c.taps);
     return cgan_conv_tc(ctx, c);
   }
-  // stride 2 (also tf.nn.conv2d_transpose of SNDCGAN's generator, arch_ops.py:588-589): input pixel 2i+a only receives
-  // the taps with kh = a + pad_t (mod 2), from output row i + (a + pad_t - kh)/2 -> four input phases in one launch
-  // (grid.z = phase), each writing a strided quarter of dx.
-  if (ctx->math_mode == 1 && d->stride == 2 && !d->upsample && d->kh * d->kw <= 16 && !(d->h & 1) && !(d->w & 1) &&
-      d->oh == d->h / 2 && d->ow == d->w / 2 && d->kh >= 2 && d->kw >= 2 &&
-      cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cout, d->cin) && ptr_ok && d->cin % 4 == 0) {
+  if (s2_phases) {
     ctx->last_path = CGAN_PATH_TCGEN05_TF32;
     if (!conv_taps_by_phase(d, 1, &c.taps))
       return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: empty phase%s", "cgan_conv2d_dgrad");
@@ -226,7 +230,9 @@ int cgan_conv2d_wgrad_ex(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x,
     TcWgrad g = {};
     bool geom = false;
     if (d->stride == 2) {
-      geom = !d->upsample && !(d->h & 1) && !(d->w & 1) && d->oh == d->h / 2 && d->ow == d->w / 2 &&
+      // an odd H gives ceil(H/2) output rows; the odd parity view of x is then one row short, and TMA zero-fills the
+      // row past it exactly where SAME padding puts a zero (tc_in_phases)
+      geom = !d->upsample && d->h >= 2 && d->w >= 2 && d->oh == (d->h + 1) / 2 && d->ow == (d->w + 1) / 2 &&
              conv_taps(d, 1, TAP_VIEW, &g.taps);
       tc_in_phases(&g.x, x, d->n, d->h, d->w, d->cin);
       tc_in_dense(&g.dy, dy, d->n, d->oh, d->ow, d->cout);

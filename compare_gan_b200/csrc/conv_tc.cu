@@ -44,7 +44,7 @@ struct TcParams {
   int bw, bh, bni;                  // tile box: bw*bh*bni == 128
   int tiles_w, tiles_h;             // tiles per image row / column
   int rows_used;                    // bw*bh*bni <= 128 pixel rows actually filled by the TMA box
-  int img_n, img_h, img_w;          // extent of the pixel grid (tiles at the border hang over; those rows are not stored)
+  int img_n;                        // images of the pixel grid (tiles at the border hang over; those rows are not stored)
   int relu;                         // fused ReLU in the epilogue
   int vec2;                         // 1: every output row starts at an even element offset and cout is even (float2 stores)
   int round_a;                      // 1: round the activation tiles to nearest TF32 in shared memory (operand not pre-rounded)
@@ -66,6 +66,7 @@ struct TcParams {
   int nphases;
   int ph_tap0[5];
   long long ph_base[4];
+  int ph_h[4], ph_w[4];             // pixels phase ph stores: rows < ph_h[ph], columns < ph_w[ph] (odd stride-2 dx: unequal)
   // halo mode (conv_tc_halo_kernel): the taps come in `hg` groups of `hnv` vertically consecutive taps that share their
   // horizontal offset; one TMA box of bh + hnv - 1 rows serves all taps of a group (the vertical shift is a descriptor
   // offset of bw rows), so the activation operand crosses L2 -> smem `hg` times per channel chunk instead of hg * hnv
@@ -113,7 +114,7 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* ac
     const int wi = m % p.bw;
     const int hi = (m / p.bw) % p.bh;
     const int ni = m / (p.bw * p.bh);
-    if (!(m < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.img_h && ow0 + wi < p.img_w)) continue;
+    if (!(m < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.ph_h[blockIdx.z] && ow0 + wi < p.ph_w[blockIdx.z])) continue;
     const long long roff = out_base + (long long)(n0 + ni) * p.s_n + (long long)(oh0 + hi) * p.s_h +
                            (long long)(ow0 + wi) * p.s_w + nb0;
 #pragma unroll
@@ -163,7 +164,7 @@ __device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const floa
     const int wi = m[h] % p.bw;
     const int hi = (m[h] / p.bw) % p.bh;
     const int ni = m[h] / (p.bw * p.bh);
-    ok[h] = m[h] < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.img_h && ow0 + wi < p.img_w;
+    ok[h] = m[h] < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.ph_h[blockIdx.z] && ow0 + wi < p.ph_w[blockIdx.z];
     roff[h] = out_base + (long long)(n0 + ni) * p.s_n + (long long)(oh0 + hi) * p.s_h + (long long)(ow0 + wi) * p.s_w + nb0;
   }
   const uint32_t bias_addr = smem_u32(s_bias);
@@ -272,7 +273,8 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
       }
       if (p.ep_smem) {
         // the residual / mask tiles, one 32-column chunk per slot of the ring: the first one lands while the consumers
-        // still run the last stages - 1 k-blocks.  Box rows past the grid are zero-filled and count in the bytes.
+        // still run the last stages - 1 k-blocks.  Box rows past the grid, or past the phase's own extent (the map of
+        // each phase has that extent), are zero-filled and count in the bytes.
         const CUtensorMap* em = &tm_e.m[blockIdx.z];
         for (int t = 0; t < nt_here; ++t) {
           int ow0, oh0, n0;
@@ -678,13 +680,17 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   // VALID convolutions shrink it, their taps only carry non-negative offsets
   tc_geometry(n, gh, gw, &p.bw, &p.bh, &p.bni, &p.tiles_w, &p.tiles_h, &tiles_n);
   p.rows_used = p.bw * p.bh * p.bni;
-  p.img_n = n; p.img_h = gh; p.img_w = gw;
+  p.img_n = n;
   p.relu = c.relu;
   p.round_a = c.a.tf32 ? 0 : 1;
   p.round_out = c.round_out; p.residual = c.residual; p.mask = c.mask; p.mask_leak = c.mask_leak;
   p.nphases = 1;
   p.ph_tap0[0] = 0; p.ph_tap0[1] = ntaps;
   p.ph_base[0] = c.base;
+  for (int i = 0; i < 4; ++i) {
+    p.ph_h[i] = c.ph_h[i] ? c.ph_h[i] : gh;
+    p.ph_w[i] = c.ph_w[i] ? c.ph_w[i] : gw;
+  }
   if (tp.nphases > 1) {
     if (tp.nphases > 4) return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: more than four phases%s", "cgan_conv_tc");
     p.nphases = tp.nphases;
@@ -821,8 +827,8 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   memset(&tm_e, 0, sizeof(tm_e));
   p.ep_smem = tc_ep_smem_ok(p, c) ? 1 : 0;
   for (int v = 0; p.ep_smem && v < p.nphases; ++v)
-    if (!make_act_map(&tm_e.m[v], (c.residual ? c.residual : c.mask) + p.ph_base[v], c.ncols, gw, gh, n, p.s_w, p.s_h,
-                      p.s_n, p.bw, p.bh, p.bni))
+    if (!make_act_map(&tm_e.m[v], (c.residual ? c.residual : c.mask) + p.ph_base[v], c.ncols, p.ph_w[v], p.ph_h[v], n,
+                      p.s_w, p.s_h, p.s_n, p.bw, p.bh, p.bni))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(residual / mask) failed%s", "cgan_conv_tc");
   size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/ + (p.ep_smem ? p.bn * 4 : 0) /*bias*/;
   dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles, (unsigned)p.nphases);

@@ -8,7 +8,7 @@
 //
 //   cin <= 4   forward   : P = patches(x) [pixels, 32]  ->  y  = P W            (1x1 wgmma conv, fused epilogue)
 //              filter    : dW = P^T dy                                            (wgmma filter-gradient kernel)
-//              input grad: T = dy W^T [pixels, 32]      ->  dx = shift_add(T)
+//              input grad: T = dy W^T [pixels, 32]      ->  dx = shift_add(T)     (stride 1 or 2)
 //   cout <= 4  forward   : T = x W' [pixels, 32]        ->  y  = shift_add(T) + bias
 //              input grad: P = patches(dy)              ->  dx = P W'^T
 //              filter    : dW' = x^T P                                            (then re-laid out to HWIO)
@@ -68,6 +68,9 @@ patch_kernel(float* __restrict__ out, const float* __restrict__ src, TapList t, 
 }
 
 // out[(n, y, x)][c] = bias[c] + sum_tap T[(n, y + off_h[tap], x + off_w[tap])][tap*C + c]   (taps outside the th x tw grid: 0)
+// STRIDE 2 (the input gradient of a stride-2 convolution): T row ((y + off_h) / 2, (x + off_w) / 2), only where both sums
+// are even; an odd one is a tap that no output pixel of the forward convolution sends to (y, x)
+template <int STRIDE>
 __global__ void shift_add_kernel(float* __restrict__ out, const float* __restrict__ t32, const float* __restrict__ bias,
                                  TapList t, int n, int oh, int ow, int th, int tw, int relu) {
   const long long total = (long long)n * oh * ow;
@@ -81,7 +84,11 @@ __global__ void shift_add_kernel(float* __restrict__ out, const float* __restric
     if (bias)
       for (int c = 0; c < t.c; ++c) acc[c] = bias[c];
     for (int tap = 0; tap < t.ntaps; ++tap) {
-      const int ty = y + t.off_h[tap], tx = x + t.off_w[tap];
+      int ty = y + t.off_h[tap], tx = x + t.off_w[tap];
+      if (STRIDE == 2) {
+        if ((ty | tx) & 1) continue;
+        ty >>= 1; tx >>= 1;
+      }
       if (ty < 0 || ty >= th || tx < 0 || tx >= tw) continue;
       const float* row = t32 + (((long long)img * th + ty) * tw + tx) * TT_K + tap * t.c;
       for (int c = 0; c < t.c; ++c) acc[c] += __ldg(row + c);
@@ -172,6 +179,9 @@ inline bool common_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
          (long long)d->n * d->oh * d->ow < (1ll << 31) && (long long)d->n * d->h * d->w < (1ll << 31);
 }
 inline bool stride1_same_grid(const cgan_conv_desc* d) { return d->stride == 1 && d->oh == d->h && d->ow == d->w; }
+inline bool stride2_same_grid(const cgan_conv_desc* d) {
+  return d->stride == 2 && d->oh == (d->h + 1) / 2 && d->ow == (d->w + 1) / 2;
+}
 
 }  // namespace
 
@@ -224,7 +234,8 @@ int cgan_thin_tc_wgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
 }
 
 bool cgan_thin_tc_dgrad_cin_ok(cgan_ctx* ctx, const cgan_conv_desc* d) {
-  return common_ok(ctx, d) && stride1_same_grid(d) && d->cin >= 1 && d->cin <= 4 && d->kh * d->kw * d->cin <= TT_K && d->cout >= 8 &&
+  return common_ok(ctx, d) && (stride1_same_grid(d) || stride2_same_grid(d)) && d->cin >= 1 && d->cin <= 4 &&
+         d->kh * d->kw * d->cin <= TT_K && d->cout >= 8 &&
          d->cout % 4 == 0 && cgan_tc_shape_ok(d->n, d->oh, d->ow, d->cout, TT_K);
 }
 
@@ -241,8 +252,12 @@ int cgan_thin_tc_dgrad_cin(cgan_ctx* ctx, const cgan_conv_desc* d, const float* 
   tc_set_epilogue(&c, nullptr, ep && (ep->flags & CGAN_CONV_IN_TF32));
   rc = cgan_conv_tc(ctx, c);
   if (rc) return rc;
-  shift_add_kernel<<<ew_blocks(ctx, (long long)d->n * d->h * d->w), 256, 0, ctx->stream>>>(dx, tt, ep ? ep->bias : nullptr, t, d->n,
-                                                                                           d->h, d->w, d->oh, d->ow, 0);
+  // dx gathers T over dy's grid: at stride 2, pixel i receives tap kh from dy row (i + pad_t - kh) / 2 when that is whole
+  const int blocks = ew_blocks(ctx, (long long)d->n * d->h * d->w);
+  if (d->stride == 2)
+    shift_add_kernel<2><<<blocks, 256, 0, ctx->stream>>>(dx, tt, ep ? ep->bias : nullptr, t, d->n, d->h, d->w, d->oh, d->ow, 0);
+  else
+    shift_add_kernel<1><<<blocks, 256, 0, ctx->stream>>>(dx, tt, ep ? ep->bias : nullptr, t, d->n, d->h, d->w, d->oh, d->ow, 0);
   CGAN_LAUNCHED(ctx);
   if (ep_needs_post(ep, false))
     return cgan_conv_post_epilogue(ctx, dx, (int64_t)d->n * d->h * d->w, d->cin, d->cin, ep->residual, ep->mask, ep->mask_leak,
@@ -273,7 +288,7 @@ int cgan_thin_tc_fwd_cout(cgan_ctx* ctx, const cgan_conv_desc* d, const float* x
   if (rc) return rc;
   const bool post = ep_needs_post(ep, true);
   const int relu = (ep && (ep->flags & CGAN_CONV_RELU)) ? 1 : 0;
-  shift_add_kernel<<<ew_blocks(ctx, pixels), 256, 0, ctx->stream>>>(y, tt, ep ? ep->bias : nullptr, t, d->n, d->oh, d->ow, d->h, d->w,
+  shift_add_kernel<1><<<ew_blocks(ctx, pixels), 256, 0, ctx->stream>>>(y, tt, ep ? ep->bias : nullptr, t, d->n, d->oh, d->ow, d->h, d->w,
                                                                    post ? 0 : relu);
   CGAN_LAUNCHED(ctx);
   if (post)

@@ -19,7 +19,11 @@ DATASETS = {
     "celeb_a_hq_128": (128, 3, None, 10000),      # named by sndcgan_celebahq128.gin:4 (SURVEY App. C note)
     "lsun-bedroom": (128, 3, None, 30000),
     "imagenet_128": (128, 3, 1000, 50000),
+    "mnist": (28, 1, 10, 10000),                   # datasets.py:332-343
+    "fashion-mnist": (28, 1, 10, 10000),           # datasets.py:346-357
 }
+# keys whose data set goes by another name (ImageDatasetV2.name, which also names the shard files)
+DATASET_NAMES = {"fashion-mnist": "fashion_mnist"}
 
 
 class ImageDatasetV2(object):
@@ -170,5 +174,5 @@ def get_dataset(name, seed=547, fake_dataset=True, data_dir=None, shuffle_buffer
   if name not in DATASETS:
     raise ValueError("Dataset %s is not available." % name)
   res, colors, classes, n_eval = DATASETS[name]
-  return ImageDatasetV2(name, res, colors, classes, n_eval, seed=seed, fake_dataset=fake_dataset, data_dir=data_dir,
+  return ImageDatasetV2(DATASET_NAMES.get(name, name), res, colors, classes, n_eval, seed=seed, fake_dataset=fake_dataset, data_dir=data_dir,
                         shuffle_buffer_size=shuffle_buffer_size)

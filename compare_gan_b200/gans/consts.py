@@ -17,6 +17,6 @@ for _name in ("infogan", "dcgan", "resnet_cifar", "sndcgan", "resnet5", "resnet3
   ARCHITECTURES.append(_name + "_arch")
 DUMMY_ARCH = "dummy_arch"          # the reference's test-only architecture name
 
-IMPLEMENTED_ARCHITECTURES = ["dcgan_arch", "resnet_cifar_arch", "sndcgan_arch", "resnet5_arch", "resnet30_arch",
+IMPLEMENTED_ARCHITECTURES = ["infogan_arch", "dcgan_arch", "resnet_cifar_arch", "sndcgan_arch", "resnet5_arch", "resnet30_arch",
                              "resnet_stl_arch", "resnet_biggan_arch", "resnet_biggan_deep_arch"]
 del _name

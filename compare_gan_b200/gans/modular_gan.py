@@ -16,8 +16,8 @@ from .. import gin_lite as gin
 from .. import kernels as K
 from .. import tape
 from .. import variables as V
-from ..architectures import (dcgan, resnet5, resnet30, resnet_biggan, resnet_biggan_deep, resnet_cifar, resnet_stl,
-                             sndcgan)
+from ..architectures import (dcgan, infogan, resnet5, resnet30, resnet_biggan, resnet_biggan_deep, resnet_cifar,
+                             resnet_stl, sndcgan)
 from ..tpu import tpu_ops
 from . import consts, loss_lib, penalty_lib
 from .abstract_gan import AbstractGAN
@@ -101,7 +101,7 @@ class ModularGAN(AbstractGAN):
       module = {consts.RESNET5_ARCH: resnet5, consts.RESNET_BIGGAN_ARCH: resnet_biggan, consts.DCGAN_ARCH: dcgan,
                 consts.RESNET_BIGGAN_DEEP_ARCH: resnet_biggan_deep,
                 consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan, consts.RESNET30_ARCH: resnet30,
-                consts.RESNET_STL_ARCH: resnet_stl}.get(self._architecture)
+                consts.RESNET_STL_ARCH: resnet_stl, consts.INFOGAN_ARCH: infogan}.get(self._architecture)
       if module is None:
         raise NotImplementedError("Architecture {} not implemented.".format(self._architecture))
       self._generator = module.Generator(image_shape=self._dataset.image_shape)
@@ -113,7 +113,7 @@ class ModularGAN(AbstractGAN):
       module = {consts.RESNET5_ARCH: resnet5, consts.RESNET_BIGGAN_ARCH: resnet_biggan, consts.DCGAN_ARCH: dcgan,
                 consts.RESNET_BIGGAN_DEEP_ARCH: resnet_biggan_deep,
                 consts.RESNET_CIFAR_ARCH: resnet_cifar, consts.SNDCGAN_ARCH: sndcgan, consts.RESNET30_ARCH: resnet30,
-                consts.RESNET_STL_ARCH: resnet_stl}.get(self._architecture)
+                consts.RESNET_STL_ARCH: resnet_stl, consts.INFOGAN_ARCH: infogan}.get(self._architecture)
       if module is None:
         raise NotImplementedError("Architecture {} not implemented.".format(self._architecture))
       self._discriminator = module.Discriminator()
