@@ -2,6 +2,7 @@
 // Replaces: the covariance/mean part of tfgan.eval.frechet_classifier_distance_from_activations
 // (metrics/fid_score.py:49-51) and tfgan.eval.preprocess_image (eval_utils.py:170-175).
 #include "common.cuh"
+#include "resize.cuh"
 
 namespace {
 
@@ -43,15 +44,10 @@ __global__ void resize_bilinear_kernel(float* __restrict__ y, const float* __res
     int ox = (int)(t % ow); t /= ow;
     int oy = (int)(t % oh);
     long long b = t / oh;
-    float fy = oy * sh, fx = ox * sw;
-    int y0 = (int)floorf(fy), x0 = (int)floorf(fx);
-    int y1 = min(y0 + 1, h - 1), x1 = min(x0 + 1, w - 1);
-    float ly = fy - y0, lx = fx - x0;
+    const TfBilinearTap ty = tf_bilinear_tap<false>(oy, sh, h), tx = tf_bilinear_tap<false>(ox, sw, w);
     const float* p = x + b * h * w * c + ch;
-    float v00 = p[((long long)y0 * w + x0) * c], v01 = p[((long long)y0 * w + x1) * c];
-    float v10 = p[((long long)y1 * w + x0) * c], v11 = p[((long long)y1 * w + x1) * c];
-    float top = v00 + (v01 - v00) * lx, bot = v10 + (v11 - v10) * lx;
-    float v = top + (bot - top) * ly;
+    float v = tf_bilinear<false>(p[((long long)ty.lo * w + tx.lo) * c], p[((long long)ty.lo * w + tx.hi) * c],
+                                 p[((long long)ty.hi * w + tx.lo) * c], p[((long long)ty.hi * w + tx.hi) * c], tx.lerp, ty.lerp);
     if (incep) v = (v * 255.0f - 128.0f) / 128.0f;
     y[i] = v;
   }

@@ -296,8 +296,8 @@ def _real_images(dataset, n_total, n_local, rank, world, batch_size):
     out, i = [], 0
     try:
       for images, _ in it:
-        if i % world == rank:
-          out.append(np.array(images, np.float32, copy=True))
+        if i % world == rank:       # (transformed sources hand out device batches)
+          out.append(images.to("cpu", copy=True).numpy() if hasattr(images, "cpu") else np.array(images, np.float32, copy=True))
         it.release(1)
         i += 1
         if sum(len(o) for o in out) >= n_local:

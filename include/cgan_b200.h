@@ -362,6 +362,30 @@ int cgan_cov_accumulate(cgan_ctx*, const float* act, int n, int d, double* sum, 
  * when `inception_scale` (eval_utils.py:157-175). */
 int cgan_resize_bilinear(cgan_ctx*, float* y, const float* x, int n, int h, int w, int c, int oh, int ow, int inception_scale);
 
+/* ---- data set transforms (ImageNet / CelebA / LSUN input transforms, datasets.py:374-427, 440-532) ---- */
+/* One element of a packed uint8 batch (cgan_loader_next_packed).  Its window, h x w pixels of c channels HWC, starts
+ * `offset` bytes into the packed batch and sits on a canvas_h x canvas_w canvas with its top-left pixel at (top, left);
+ * canvas pixels outside the window are 0 (tf.image.resize_image_with_crop_or_pad's padding).  position is the element's
+ * place p in the repeated stream, element its source index, (crop_y, crop_x) the window's origin in the source image. */
+typedef struct cgan_crop_desc {
+  int64_t offset;
+  int64_t position;
+  int32_t element;
+  int32_t h, w;
+  int32_t canvas_h, canvas_w;
+  int32_t top, left;
+  int32_t crop_y, crop_x;
+  int32_t reserved;
+} cgan_crop_desc;
+/* out [n, r, r, c] fp32 NHWC: each element's canvas resized to r x r by TF1's legacy bilinear resize
+ * (tf.image.resize_images: align_corners = False, src = dst * (in / out), no half-pixel offset), every operation a
+ * separately rounded fp32 operation (no FMA contraction).  divide_after = 0 divides each uint8 tap by 255 before the
+ * interpolation (ImageNet: tf.cast / 255, then resize), 1 interpolates the uint8 values and divides the result by 255
+ * (CelebA: resize, then / 255); both are true divisions.  packed: device bytes of the batch, desc [n] device descriptors
+ * (their offsets count from `packed`); c is 1 or 3. */
+int cgan_crop_resize_u8(cgan_ctx*, float* out, const uint8_t* packed, const cgan_crop_desc* desc, int n, int c, int r,
+                        int divide_after);
+
 /* ---- MS-SSIM terms (metrics/image_similarity.py:85-211, 239-333) ---- */
 /* Per-scale SSIM terms of image pairs of ONE image set.  images [n,h,w,c] fp32 NHWC, values in [0, max_val];
  * host_pairs [npairs,2] int32 HOST indices into the set (they travel to the device in the kernel parameters, so the call
@@ -475,6 +499,45 @@ int cgan_loader_next(cgan_loader*, const float** images, const int32_t** labels)
 int cgan_loader_release(cgan_loader*, int count);
 int cgan_loader_destroy(cgan_loader*);
 const char* cgan_loader_last_error(cgan_loader*);
+
+/* Sources of any image size for the transformed path: n images of c channels, image i being index[i] = (offset, h, w)
+ * row-major HWC uint8 at pixels + offset (host memory, caller-owned, must outlive the loader), and optional int32
+ * labels. */
+typedef struct cgan_image_source {
+  const uint8_t* pixels;
+  int64_t pixel_bytes;
+  const int64_t* index;
+  const int32_t* labels;
+  int64_t n;
+  int32_t c;
+  int32_t reserved;
+} cgan_image_source;
+enum { CGAN_CROP_NONE = 0, CGAN_CROP_MIDDLE = 1, CGAN_CROP_RANDOM = 2, CGAN_CROP_DISTORTED = 3, CGAN_CROP_OR_PAD = 4 };
+enum { CGAN_LABEL_SOURCE = 0, CGAN_LABEL_ZERO = 1, CGAN_LABEL_RANDOM = 2 };
+/* The per-element transform (datasets.py:374-427, 440-584).  crop: CGAN_CROP_* (datasets.py:458-491; CGAN_CROP_OR_PAD is
+ * tf.image.resize_image_with_crop_or_pad to canvas_h x canvas_w).  Filters, applied once at creation (an empty element
+ * list is an error): min_side > 0 keeps images with min(h, w) >= min_side, labeled_only keeps labels >= 0.  label:
+ * CGAN_LABEL_SOURCE (0 without source labels), CGAN_LABEL_ZERO, or CGAN_LABEL_RANDOM (uniform in [0, random_classes),
+ * drawn anew for every stream position). */
+typedef struct cgan_image_transform {
+  int32_t crop;
+  int32_t canvas_h, canvas_w;
+  int32_t min_side;
+  int32_t labeled_only;
+  int32_t label;
+  int32_t random_classes;
+  int32_t reserved;
+} cgan_image_transform;
+/* A loader whose producer packs, per element, only the rows of the element's crop window: each ring slot holds the
+ * batch's cgan_crop_desc table ([batch] descriptors at the start of the slot) followed by the packed window bytes, ready
+ * for ONE host->device copy and cgan_crop_resize_u8.  The element of stream position p is list[p % n] (list: the filtered
+ * source indices, in source order); the shuffle is cgan_loader_create's.  Random crops and labels are keyed by
+ * (seed, p, draw index) through SplitMix64, so they depend on neither the shuffle buffer nor thread timing. */
+int cgan_loader_create_transformed(cgan_loader** out, const cgan_image_source* source, const cgan_image_transform* transform,
+                                   int batch, int shuffle_buffer, uint64_t seed, int ring);
+/* cgan_loader_next for a transformed loader: *slot_data points at the slot ([batch] descriptors, then the packed bytes),
+ * *slot_bytes is the size of what the batch used, labels int32 [batch]. */
+int cgan_loader_next_packed(cgan_loader*, const uint8_t** slot_data, int64_t* slot_bytes, const int32_t** labels);
 
 #ifdef __cplusplus
 }
