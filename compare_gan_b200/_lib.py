@@ -29,6 +29,7 @@ CONV_RELU, CONV_ROUND_OUT, CONV_IN_TF32, CONV_IN2_TF32 = 1, 2, 4, 8
 ACT_ROUND_TF32 = 0x100
 OPT_TC_MT, OPT_LAST_PATH, OPT_TC_HALO, OPT_TC_THIN = 1, 2, 3, 6
 OPT_LAST_TC_BN, OPT_LAST_TC_MT, OPT_LAST_TC_HALO, OPT_LAST_TC_CTAS_PER_SM, OPT_LAST_TC_EP_SMEM = 7, 8, 9, 10, 11
+OPT_LAST_TC_TMA_STORE = 12
 PATH_NAMES = {0: "simt_fp32", 1: "tcgen05_tf32", 2: "thin_fp32"}
 
 _SCALARS = {"int": ctypes.c_int, "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64,

@@ -22,6 +22,7 @@ struct cgan_ctx {
   int last_tc_bn, last_tc_mt, last_tc_halo;   // geometry of the most recent conv_tc launch (CGAN_OPT_LAST_TC_*)
   int last_tc_ctas_per_sm;                    // CTAs of that launch that fit on one SM (CGAN_OPT_LAST_TC_CTAS_PER_SM)
   int last_tc_ep_smem;                        // that launch prefetched its residual / mask (CGAN_OPT_LAST_TC_EP_SMEM)
+  int last_tc_tma_store;                      // that launch stored its tiles by TMA (CGAN_OPT_LAST_TC_TMA_STORE)
   unsigned* counters;  // CGAN_NUM_COUNTERS zero-initialised tickets for single-launch two-stage reductions (norm.cu)
   void* p2p;           // peer-memory all-reduce state (p2p.cu), null until cgan_p2p_local_handle
   char err[512];

@@ -12,12 +12,13 @@
 //   MMAs read them — the tensor core would otherwise truncate the low 13 bits, a systematic -2^-11 relative bias per
 //   product that accumulates through a 13-layer discriminator.
 // * Warp roles: warps 0..7 = two consumer warpgroups, warpgroup g owning rows 64g..64g+63 of every 128-pixel tile:
-//   (operand rounding,) wgmma m64nBNk8 (K = 8 per instruction, fp32 accumulators in registers), epilogue straight from
-//   the accumulator fragments (+bias, residual, ReLU / mask, TF32 rounding -> global); warp 8 = TMA producer.
+//   (operand rounding,) wgmma m64nBNk8 (K = 8 per instruction, fp32 accumulators in registers), epilogue from the
+//   accumulator fragments (+bias, residual, ReLU / mask, TF32 rounding); warp 8 = TMA producer.
 //   Stages are released one k-block late (wgmma.wait_group 1), so the rounding of the next stage overlaps the MMAs.
-// * A residual or ReLU mask (tensors of the output's geometry, far larger than L2 in a training step) is not read by
-//   the epilogue from global memory: after its last k-block the producer goes on around the stage ring and TMA-loads the
-//   CTA's tile of it, one 32-column chunk per stage, while the consumers finish their MMAs.
+// * The epilogue of a float2 launch goes through the stage ring (tile_epilogue_smem): after its last k-block the
+//   producer goes on around the ring, one 32-column chunk of the CTA's tile per slot, TMA-loading the chunk of a residual
+//   or ReLU mask (tensors of the output's geometry, far larger than L2 in a training step) where the launch has one.
+//   The consumers write the finished chunk into the slot, and one thread TMA-stores it to the output.
 //
 // The same kernel serves forward and input-gradient convolutions (and the four sub-pixel phases of a
 // conv over a zero-inserted 2x upsampled input): the host supplies, per tap, the input offset and the weight
@@ -75,11 +76,12 @@ struct TcParams {
   int a_halo_bytes;                 // smem footprint of one tile's halo box (1024-aligned)
   int a_box_bytes;                  // bytes TMA writes per halo box
   int sa_stages, sb_stages;
-  int ep_smem;                      // 1: the residual or mask is prefetched into the stage ring (tile_epilogue_smem)
+  int ep_tma;                       // 1: the tile is staged in the stage ring and TMA-stored (tile_epilogue_smem)
+  int ep_smem;                      // 1: with ep_tma, the residual or mask is prefetched into the ring as well
 };
 
 // up to four views of the input tensor (the sub-pixel phases of a 2x-upsampled gradient); plain convs use view 0.  The
-// same holds views of the residual / mask, one per output phase.
+// same holds views of the residual / mask and of the output, one per output phase.
 struct AMaps { CUtensorMap m[4]; };
 
 
@@ -141,33 +143,26 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* ac
   }
 }
 
-// The same epilogue for a launch whose residual or mask (never both) the producer prefetched into the stage ring: the
-// 32-column chunk cc of the tile arrives in the next slot as a [rows_used][32] box, 128B-swizzled, rows in the tile's
-// pixel order.  The bias of the CTA's columns sits in shared memory.  No global load is left between two stores, so the
-// stores of a tile issue back to back instead of each waiting for its own residual / mask load.  A slot that a later
-// chunk of this CTA needs is released as soon as both warpgroups have read it.  The arithmetic and its order are
-// tile_epilogue's.
+// The same epilogue for a float2 launch with at most one of residual / mask, staged through the stage ring: chunk cc
+// (32 columns) of the tile is a [rows_used][32] box in the next slot, 128B-swizzled, rows in the tile's pixel order.
+// The producer fills the slot with the chunk of the residual or mask, or just hands it over when there is none.  Each
+// thread finishes its elements at their swizzled addresses (bias from shared memory; the arithmetic and its order are
+// tile_epilogue's), and thread 0 stores the box with one TMA store through the output map of the CTA's phase.  The map
+// clips the rows past the grid or the phase's extent and the columns past cout, so no element needs a predicate or a
+// global address.  Thread 0 hands a slot back to the producer once the store that reads it has read it and a later
+// chunk of this CTA needs it: after issuing the store of chunk k it waits for the store of chunk k - 1 (issued one
+// chunk earlier, normally done reading by then) and releases that slot, so the producer can load chunk k - 1 + stages
+// while chunk k + 1 is being finished.
 template <int BN>
-__device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const float* acc, int tile, int nb0, int wg, int warp,
-                                                 int lane, long long out_base, const uint8_t* smem, int stage_bytes,
+__device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const CUtensorMap* om, const float* acc, int tile,
+                                                 int nb0, int wg, int warp, int lane, const uint8_t* smem, int stage_bytes,
                                                  uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
-                                                 int& chunk, int chunks, const float* s_bias) {
+                                                 int& chunk, int chunks, uint32_t bias_addr) {
   int ow0, oh0, n0;
   tc_tile_origin(p, tile, ow0, oh0, n0);
   const int c2 = (lane & 3) * 2;
-  bool ok[2];
-  long long roff[2];
-  int m[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    m[h] = wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
-    const int wi = m[h] % p.bw;
-    const int hi = (m[h] / p.bw) % p.bh;
-    const int ni = m[h] / (p.bw * p.bh);
-    ok[h] = m[h] < p.rows_used && n0 + ni < p.img_n && oh0 + hi < p.ph_h[blockIdx.z] && ow0 + wi < p.ph_w[blockIdx.z];
-    roff[h] = out_base + (long long)(n0 + ni) * p.s_n + (long long)(oh0 + hi) * p.s_h + (long long)(ow0 + wi) * p.s_w + nb0;
-  }
-  const uint32_t bias_addr = smem_u32(s_bias);
+  const int m0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const bool operand = p.residual || p.mask;
 #pragma unroll
   for (int cc = 0; cc < BN / 32; ++cc) {
     mbar_wait(&full_bar[stage], phase);
@@ -175,25 +170,27 @@ __device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const floa
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const int j = cc * 4 + jj, c = j * 8 + c2;
-      if (nb0 + c >= p.cout) continue;
       const float2 b = p.bias ? lds64(bias_addr + c * 4) : make_float2(0.f, 0.f);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (!ok[h]) continue;
+        const uint32_t a = e_addr + sw128_offset(m0 + h * 8, jj * 8 + c2);
         float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        const float2 e = lds64(e_addr + sw128_offset(m[h], jj * 8 + c2));
+        const float2 e = operand ? lds64(a) : make_float2(0.f, 0.f);
         if (p.bias) { v.x += b.x; v.y += b.y; }
         if (p.residual) { v.x += e.x; v.y += e.y; }
         if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
         if (p.mask) { v.x = e.x > 0.f ? v.x : p.mask_leak * v.x; v.y = e.y > 0.f ? v.y : p.mask_leak * v.y; }
         if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
-        *reinterpret_cast<float2*>(p.out + roff[h] + c) = v;
+        sts64(a, v);
       }
     }
-    if (chunk + p.stages < chunks) {           // a later chunk of this CTA refills the slot
-      fence_proxy_async();
-      named_bar(1 + wg, 128);
-      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+    fence_proxy_async();                       // the chunk's writes become visible to the TMA store
+    named_bar(3, 32 * TC_CWARPS);
+    if (threadIdx.x == 0) {
+      tma_store_4d(om, e_addr, nb0 + cc * 32, ow0, oh0, n0);
+      bulk_commit();
+      bulk_wait_read<1>();                     // the store of chunk - 1 has read its slot
+      if (chunk >= 1 && chunk - 1 + p.stages < chunks) mbar_arrive(&empty_bar[stage == 0 ? p.stages - 1 : stage - 1], 2);
     }
     ++chunk;
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -218,9 +215,9 @@ __device__ __forceinline__ void tc_round_smem(uint32_t base, int bytes, int q, i
 template <int BN, int MT>
 __global__ void __launch_bounds__(TC_THREADS, tc_min_ctas(BN, MT))
 conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUtensorMap tm_b, const TcParams p,
-               const __grid_constant__ AMaps tm_e) {
+               const __grid_constant__ AMaps tm_e, const __grid_constant__ AMaps tm_o) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][MT x A 16KB][B BN*128B] | barriers (256 B) | with ep_smem: the bias of the CTA's BN columns
+  // carve: [stages][MT x A 16KB][B BN*128B] | barriers (256 B) | with ep_tma: the bias of the CTA's BN columns
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int b_bytes = BN * TC_BK * 4;
   constexpr int a_bytes = MT * TC_A_BYTES;
@@ -271,18 +268,23 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
         tma_load_3d(sb, &tm_b, &full_bar[stage], kc * TC_BK, nb0, p.wtap[tap] + n0 * p.wimg_stride);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-      if (p.ep_smem) {
-        // the residual / mask tiles, one 32-column chunk per slot of the ring: the first one lands while the consumers
-        // still run the last stages - 1 k-blocks.  Box rows past the grid, or past the phase's own extent (the map of
-        // each phase has that extent), are zero-filled and count in the bytes.
+      if (p.ep_tma) {
+        // the epilogue's slots, one per 32-column chunk of the CTA's tiles: the first one is handed over while the
+        // consumers still run the last stages - 1 k-blocks.  With a residual / mask the chunk of it is loaded into the
+        // slot; box rows past the grid, or past the phase's own extent (the map of each phase has that extent), are
+        // zero-filled and count in the bytes.
         const CUtensorMap* em = &tm_e.m[blockIdx.z];
         for (int t = 0; t < nt_here; ++t) {
           int ow0, oh0, n0;
           tc_tile_origin(p, tile0 + t, ow0, oh0, n0);
           for (int cc = 0; cc < BN / 32; ++cc) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_expect_tx(&full_bar[stage], (uint32_t)(p.rows_used * TC_BK * 4));
-            tma_load_4d(smem + stage * stage_bytes, em, &full_bar[stage], nb0 + cc * 32, ow0, oh0, n0);
+            if (p.ep_smem) {
+              mbar_expect_tx(&full_bar[stage], (uint32_t)(p.rows_used * TC_BK * 4));
+              tma_load_4d(smem + stage * stage_bytes, em, &full_bar[stage], nb0 + cc * 32, ow0, oh0, n0);
+            } else {
+              mbar_arrive(&full_bar[stage]);
+            }
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
         }
@@ -292,7 +294,7 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
     // ===== consumer warpgroups =====
     const int wg = warp >> 2;
     const int q = threadIdx.x & 127;
-    if (p.ep_smem && p.bias)
+    if (p.ep_tma && p.bias)
       for (int i = threadIdx.x; i < BN; i += 32 * TC_CWARPS) s_bias[i] = nb0 + i < p.cout ? p.bias[nb0 + i] : 0.f;
     float acc[MT][BN / 2];
 #pragma unroll
@@ -334,8 +336,8 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
-    if (p.ep_smem) {
-      // the last k-block's stage goes back to the producer for the residual / mask chunks
+    if (p.ep_tma) {
+      // the last k-block's stage goes back to the producer for the epilogue's chunks
       if (prev >= 0 && q == 0) mbar_arrive(&empty_bar[prev]);
       named_bar(3, 32 * TC_CWARPS);              // s_bias is written
       int chunk = 0;
@@ -344,9 +346,10 @@ conv_tc_kernel(const __grid_constant__ AMaps tm_as, const __grid_constant__ CUte
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc_fence(acc[t][i]);
         if (t < nt_here)
-          tile_epilogue_smem<BN>(p, acc[t], tile0 + t, nb0, wg, warp, lane, p.ph_base[blockIdx.z], smem, stage_bytes,
-                                 full_bar, empty_bar, stage, phase, chunk, nt_here * (BN / 32), s_bias);
+          tile_epilogue_smem<BN>(p, &tm_o.m[blockIdx.z], acc[t], tile0 + t, nb0, wg, warp, lane, smem, stage_bytes,
+                                 full_bar, empty_bar, stage, phase, chunk, nt_here * (BN / 32), smem_u32(s_bias));
       }
+      if (threadIdx.x == 0) bulk_wait_read<0>();   // the ring stays allocated until the last store has read it
     } else {
 #pragma unroll
       for (int t = 0; t < MT; ++t) {
@@ -570,16 +573,23 @@ inline int tc_vec2(const TcParams& p) {
   return (odd & 1) ? 0 : 1;
 }
 
-// The per-tap kernel prefetches the residual or the mask of a launch (tile_epilogue_smem) when it has one of them, not
-// both, and TMA can read it in the output's geometry: every phase's first element and the pixel strides 16-byte aligned,
-// and the float2 epilogue applies.  Any other launch reads its epilogue operands from global memory in tile_epilogue.
-inline bool tc_ep_smem_ok(const TcParams& p, const TcConv& c) {
+// The per-tap kernel stages its epilogue through the stage ring and stores the tiles by TMA (tile_epilogue_smem) when the
+// float2 epilogue applies, the launch has at most one of residual / mask, and TMA can address the output (and that
+// operand) in the output's geometry: bases, every phase's first element and the pixel strides 16-byte aligned.  Any
+// other launch (a channel slice at an unaligned offset or width, residual and mask together) keeps tile_epilogue.
+inline bool tc_ep_tma_ok(const TcParams& p, const TcConv& c) {
   const float* e = c.residual ? c.residual : c.mask;
-  if (!e || (c.residual && c.mask) || !p.vec2 || (reinterpret_cast<uintptr_t>(e) & 15)) return false;
+  if (!p.vec2 || (c.residual && c.mask) || ((reinterpret_cast<uintptr_t>(c.out) | reinterpret_cast<uintptr_t>(e)) & 15))
+    return false;
   long long a = p.s_n | p.s_h | p.s_w;
   for (int i = 0; i < p.nphases; ++i) a |= p.ph_base[i];
   return (a & 3) == 0;
 }
+
+// Kernel parameters of conv_tc_kernel, within the 4 KB a launch may pass: three AMaps (activation views, residual /
+// mask views, output views) of 4 x 128 B, one 128 B weight map and TcParams, plus at most 2 x 63 B of padding in front
+// of the 64-byte aligned maps after TcParams.
+static_assert(3 * sizeof(AMaps) + sizeof(CUtensorMap) + sizeof(TcParams) + 2 * 63 <= 4096, "conv_tc_kernel parameters");
 
 // Weights -> TF32-rounded (nearest) K-major [taps_total][ncols_pad][kdim_pad] in the context workspace
 int prep_weights(cgan_ctx* ctx, const TcConv& c, int kdim_pad, int ncols_pad, float** out) {
@@ -618,7 +628,7 @@ int tc_ctas_per_sm(Kernel kernel, size_t smem) {
 // halo: the halo kernel, reading the activation box through as.m[0]
 template <int BN, int MT>
 int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p,
-                const AMaps& es) {
+                const AMaps& es, const AMaps& os) {
   static bool attr_set[2] = {false, false};
   if (halo) {
     if (!attr_set[1]) {
@@ -633,19 +643,20 @@ int tc_launch_t(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& a
       attr_set[0] = true;
     }
     ctx->last_tc_ctas_per_sm = tc_ctas_per_sm(conv_tc_kernel<BN, MT>, smem);
-    conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p, es);
+    conv_tc_kernel<BN, MT><<<grid, TC_THREADS, smem, ctx->stream>>>(as, b, p, es, os);
   }
   CGAN_LAUNCHED(ctx);
   return CGAN_OK;
 }
 
 // the accumulator fragment is sized at compile time: one instantiation per (bn, mt), mt * bn <= TC_ACC_COLS.  es: the
-// residual / mask views of a launch with ep_smem (unused otherwise)
+// residual / mask views of a launch with ep_smem, os: the output views of a launch with ep_tma (unused otherwise)
 int tc_launch(cgan_ctx* ctx, bool halo, dim3 grid, size_t smem, const AMaps& as, const CUtensorMap& b, const TcParams& p,
-              const AMaps& es) {
+              const AMaps& es, const AMaps& os) {
   ctx->last_tc_bn = p.bn; ctx->last_tc_mt = p.mt; ctx->last_tc_halo = halo ? 1 : 0; ctx->last_tc_ep_smem = p.ep_smem;
+  ctx->last_tc_tma_store = p.ep_tma;
 #define TC_CASE(BN, MT) \
-  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p, es);
+  if (p.bn == BN && p.mt == MT) return tc_launch_t<BN, MT>(ctx, halo, grid, smem, as, b, p, es, os);
   TC_CASE(32, 1) TC_CASE(64, 1) TC_CASE(96, 1) TC_CASE(128, 1) TC_CASE(160, 1) TC_CASE(192, 1) TC_CASE(224, 1)
   TC_CASE(256, 1) TC_CASE(32, 2) TC_CASE(64, 2) TC_CASE(96, 2) TC_CASE(128, 2)
 #undef TC_CASE
@@ -785,7 +796,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
         p.vec2 = tc_vec2(p);
         size_t smem = (size_t)p.sa_stages * p.mt * p.a_halo_bytes + (size_t)p.sb_stages * b_bytes + 1024 + 512;
         dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles);
-        return tc_launch(ctx, true, grid, smem, tm_a, tm_b, p, tm_a);
+        return tc_launch(ctx, true, grid, smem, tm_a, tm_b, p, tm_a, tm_a);
       }
     }
     // not eligible after all: restore the standard geometry
@@ -823,14 +834,20 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   if (p.stages > TC_MAX_STAGES) p.stages = TC_MAX_STAGES;
   if (p.stages < 2) p.stages = 2;
   p.vec2 = tc_vec2(p);
-  AMaps tm_e;
+  AMaps tm_e, tm_o;
   memset(&tm_e, 0, sizeof(tm_e));
-  p.ep_smem = tc_ep_smem_ok(p, c) ? 1 : 0;
-  for (int v = 0; p.ep_smem && v < p.nphases; ++v)
-    if (!make_act_map(&tm_e.m[v], (c.residual ? c.residual : c.mask) + p.ph_base[v], c.ncols, p.ph_w[v], p.ph_h[v], n,
-                      p.s_w, p.s_h, p.s_n, p.bw, p.bh, p.bni))
+  memset(&tm_o, 0, sizeof(tm_o));
+  p.ep_tma = tc_ep_tma_ok(p, c) ? 1 : 0;
+  p.ep_smem = p.ep_tma && (c.residual || c.mask) ? 1 : 0;
+  for (int v = 0; p.ep_tma && v < p.nphases; ++v) {
+    if (!make_act_map(&tm_o.m[v], c.out + p.ph_base[v], c.ncols, p.ph_w[v], p.ph_h[v], n, p.s_w, p.s_h, p.s_n, p.bw, p.bh,
+                      p.bni))
+      return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(output) failed%s", "cgan_conv_tc");
+    if (p.ep_smem && !make_act_map(&tm_e.m[v], (c.residual ? c.residual : c.mask) + p.ph_base[v], c.ncols, p.ph_w[v],
+                                   p.ph_h[v], n, p.s_w, p.s_h, p.s_n, p.bw, p.bh, p.bni))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled(residual / mask) failed%s", "cgan_conv_tc");
-  size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/ + (p.ep_smem ? p.bn * 4 : 0) /*bias*/;
+  }
+  size_t smem = (size_t)p.stages * stage_bytes + 1024 /*align*/ + 256 /*barriers*/ + (p.ep_tma ? p.bn * 4 : 0) /*bias*/;
   dim3 grid((unsigned)((tiles_total + p.mt - 1) / p.mt), (unsigned)ncol_tiles, (unsigned)p.nphases);
-  return tc_launch(ctx, false, grid, smem, tm_as, tm_b, p, tm_e);
+  return tc_launch(ctx, false, grid, smem, tm_as, tm_b, p, tm_e, tm_o);
 }

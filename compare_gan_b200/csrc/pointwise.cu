@@ -100,6 +100,7 @@ int cgan_ctx_get_option(cgan_ctx* ctx, int key, int64_t* host_value) {
     case CGAN_OPT_LAST_TC_HALO: *host_value = ctx->last_tc_halo; return CGAN_OK;
     case CGAN_OPT_LAST_TC_CTAS_PER_SM: *host_value = ctx->last_tc_ctas_per_sm; return CGAN_OK;
     case CGAN_OPT_LAST_TC_EP_SMEM: *host_value = ctx->last_tc_ep_smem; return CGAN_OK;
+    case CGAN_OPT_LAST_TC_TMA_STORE: *host_value = ctx->last_tc_tma_store; return CGAN_OK;
     default:
       return cgan_fail(ctx, CGAN_ERR_ARG, "%s: unknown option%s", "cgan_ctx_get_option");
   }

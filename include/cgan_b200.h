@@ -61,10 +61,13 @@ int64_t cgan_launch_count(cgan_ctx* ctx);
  *                       calculator reports it; 0 before the first one.
  *   CGAN_OPT_LAST_TC_EP_SMEM
  *                       (get) 1 when that launch had its residual or ReLU mask prefetched into shared memory by TMA, 0
- *                       when its epilogue read them (if any) from global memory; 0 before the first one. */
+ *                       when its epilogue read them (if any) from global memory; 0 before the first one.
+ *   CGAN_OPT_LAST_TC_TMA_STORE
+ *                       (get) 1 when that launch staged its output tiles in shared memory and stored them by TMA, 0 when
+ *                       its epilogue stored them from registers; 0 before the first one. */
 enum { CGAN_OPT_TC_MT = 1, CGAN_OPT_LAST_PATH = 2, CGAN_OPT_TC_HALO = 3, CGAN_OPT_TC_THIN = 6, CGAN_OPT_LAST_TC_BN = 7,
        CGAN_OPT_LAST_TC_MT = 8, CGAN_OPT_LAST_TC_HALO = 9, CGAN_OPT_LAST_TC_CTAS_PER_SM = 10,
-       CGAN_OPT_LAST_TC_EP_SMEM = 11 };
+       CGAN_OPT_LAST_TC_EP_SMEM = 11, CGAN_OPT_LAST_TC_TMA_STORE = 12 };
 /* CGAN_PATH_TCGEN05_TF32 keeps its name for ABI compatibility: the TF32 tensor-core (wgmma) path. */
 enum { CGAN_PATH_SIMT_FP32 = 0, CGAN_PATH_TCGEN05_TF32 = 1, CGAN_PATH_THIN_FP32 = 2 };
 int cgan_ctx_set_option(cgan_ctx* ctx, int key, int64_t value);
