@@ -5,7 +5,7 @@ The reference obtains `pool_3:0` (2048-d) and `logits:0` (1008-d) from TF-GAN's 
 available offline, so the WEIGHTS here are deterministic synthetic values (He-normal, BN folded into a per-channel
 bias) of the exact topology — throughput and the FID/IS arithmetic are exercised faithfully, absolute scores versus the
 real Inception are "parity unpinned" (SURVEY.md §7 item 7).  `load_weights` accepts a real weight dict
-(`inception/<layer>/kernel|bias`, HWIO) when one is available.
+(`inception/<layer>/kernel|bias`, HWIO) when one is available; `inception_graph.py` makes one from TF-GAN's frozen graph.
 """
 import numpy as np
 
