@@ -4,13 +4,18 @@
 //
 // A GEMM whose reduction dimension is the PIXEL index, so both operands are "MN-major" as they lie in HBM (NHWC:
 // channels contiguous): D[ci, co] += A[ci, pix] * B[pix, co].  Per k-block of 32 pixels, TMA brings
-//   * 4 boxes  [32 pixels x 32 ci]  of X  (shifted by the tap offset; SAME padding = TMA zero fill), and
-//   * N/32 boxes [32 pixels x 32 co] of dY
-// each box = 32 rows x 128 B, unswizzled.  wgmma takes 32-bit operands only K-major, so the two consumer warpgroups
-// transpose both operands into 128B-swizzled K-major tiles (one 128-byte row of 32 pixels per channel), rounding them to
-// nearest TF32 on the way, into one of two transposed buffers; the TMA stage is released as soon as it has been read.
-// Four wgmma m64nNk8 per warpgroup (K = 8 pixels) consume a k-block; warpgroup g owns ci rows 64g..64g+63.  The
-// transposition of k-block kb + 1 runs while the MMAs of kb are in flight.
+//   * 4 boxes  [32 pixels x 32 ci]  of X per (tap, ci-tile) unit (shifted by the tap offset; SAME padding = TMA zero
+//     fill), 128B-swizzled, and
+//   * N/32 boxes [32 pixels x 32 co] of dY, unswizzled,
+// each box = 32 rows x 128 B.  wgmma takes 32-bit shared-memory operands only K-major, so X goes to the MMAs from
+// registers: each consumer thread loads its m64k8 A fragments (two adjacent ci, one pixel per LDS.64) straight out of the
+// TMA stage, conflict-free thanks to the swizzle, and rounds them to nearest TF32 there.  Only dY is transposed by the
+// two consumer warpgroups into a 128B-swizzled K-major tile (one 128-byte row of 32 pixels per co), rounded on the way,
+// into one of two buffers; the TMA stage is released once its fragments are loaded and its dY transposed.  Four wgmma
+// m64nNk8 per unit and warpgroup (K = 8 pixels) consume a k-block, in two commit groups: the fragments of one group are
+// loaded while the other's MMAs run; warpgroup g owns ci rows 64g..64g+63 of each unit.
+// Per k-block of wgrad_tc_kernel<128, 2> that is 48 KB of TMA writes, 32 KB of fragment loads, 16 + 16 KB of dY
+// transpose and 64 KB of wgmma B reads, 176 KB of shared-memory traffic where transposing X as well took 240 KB.
 // The pixel range is split across CTAs (split-K); partial tiles go to a workspace and are summed in a fixed order
 // (deterministic), replacing TF's Conv2DBackpropFilter.
 // A conv over a zero-inserted 2x-upsampled input (resnet_ops.py:35-56) is handled through four strided TMA views of dY
@@ -29,7 +34,7 @@ constexpr int WG_P = 32;                 // pixels per k-block
 constexpr int WG_BOX = WG_P * 128;       // 4 KB: 32 pixel rows x 32 channels fp32
 constexpr int WG_A_BYTES = 4 * WG_BOX;   // 128 input channels
 constexpr int WG_CWARPS = 8;             // two consumer warpgroups
-constexpr int WG_THREADS = 32 * WG_CWARPS + 32;    // + the TMA producer warp
+constexpr int WG_THREADS = 32 * WG_CWARPS + 128;   // + the producer warpgroup, one thread of which issues the TMA
 constexpr int WG_MAX_TAPS = 16;
 constexpr int WG_ACC_COLS = 256;         // mt x bn accumulator columns per CTA
 
@@ -75,6 +80,34 @@ __device__ __forceinline__ void wg_transpose(uint32_t dst, uint32_t src, bool ro
   }
 }
 
+// A operand of the m64nNk8 MMAs straight from the TMA stage.  The X boxes land 128B-swizzled: pixel row p at p * 128 B,
+// its 16-byte chunk of channels 4c..4c+3 at chunk c ^ (p & 7).  Thread (warp, lane) feeds accumulator rows lane / 4 and
+// lane / 4 + 8 of its warp's 16; they are the adjacent channels cib, cib + 1 of box 2 * wg + (warp & 3) / 2, so one LDS.64
+// per pixel gives a[0], a[1] (pixel 8k + lane % 4) and one more a[2], a[3] (4 pixels on).  A half-warp's 16 lanes read
+// 4 pixels x 4 channel pairs from two chunks 16 channels apart (cib / 4 differs in bit 2), which the swizzle spreads over
+// all eight chunk positions: every LDS.64 takes the minimum two wavefronts.  Warp parity picks the other four chunks.
+// keeps the compiler from sinking a fragment's rounding past wgmma.fence
+__device__ __forceinline__ void frag_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+
+__device__ __forceinline__ int wg_a_channel(int warp, int lane) {
+  const int r = lane >> 2;
+  return 4 * (2 * (warp & 1) + (r >> 2) + 4 * ((r >> 1) & 1)) + 2 * (r & 1);
+}
+
+// the A fragments of GK consecutive k-steps, the first at src (a unit's boxes + k-step * 1024 B), rounded to nearest
+// TF32 unless the operand is pre-rounded
+template <int GK>
+__device__ __forceinline__ void wg_load_a(uint32_t (&f)[GK][4], uint32_t src, uint32_t lo, uint32_t hi, bool round) {
+#pragma unroll
+  for (int e = 0; e < GK; ++e) {
+    float2 a = lds64(src + e * 1024 + lo), b = lds64(src + e * 1024 + hi);
+    if (round) { a.x = rna_tf32(a.x); a.y = rna_tf32(a.y); b.x = rna_tf32(b.x); b.y = rna_tf32(b.y); }
+    f[e][0] = __float_as_uint(a.x); f[e][1] = __float_as_uint(a.y); f[e][2] = __float_as_uint(b.x); f[e][3] = __float_as_uint(b.y);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) frag_fence(f[e][i]);    // rounded here, not next to the MMAs
+  }
+}
+
 // PART: the box holds fewer than 32 pixels (box_any); box32's grids run the PART = false instantiations
 template <int BN, int MT, bool PART>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -84,10 +117,11 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   constexpr int b_bytes = (BN / 32) * WG_BOX;
   constexpr int a_bytes = MT * WG_A_BYTES;
   constexpr int stage_bytes = a_bytes + b_bytes;
-  // [stages] TMA ring | [2] transposed K-major operands (same sizes) | barriers
+  // [stages] TMA ring | [2] transposed K-major dY tiles | barriers
   uint8_t* tbuf = smem + p.stages * stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tbuf + 2 * stage_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tbuf + 2 * b_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
+  uint64_t* buf_free = empty_bar + p.stages;    // [2] both warpgroups' MMAs reading dY buffer b have retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work units (tap, ci tile); this CTA owns units [u0, u0 + nu) — they all contract against the same dY tile, which is
@@ -108,11 +142,12 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], WG_CWARPS);      // one arrive per consumer warp
     }
+    for (int b = 0; b < 2; ++b) mbar_init(&buf_free[b], WG_CWARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (PART) {
     // a box of fewer than 32 pixels fills the same leading rows of every 4 KB box slot of the ring: zero the others once,
-    // so the transposition feeds zeros to the MMAs of the k-block's missing pixels
+    // so the A fragments and the transposed dY tile hold zeros for the k-block's missing pixels
     const int tail = (WG_P - p.rows_used) * 128;
     const int words = p.stages * (stage_bytes / WG_BOX) * (tail / 16);
     for (int i = threadIdx.x; i < words; i += WG_THREADS) {
@@ -122,8 +157,12 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   }
   __syncthreads();
 
-  if (warp == WG_CWARPS) {
-    if (lane == 0) {
+  // a 256-column accumulator (128 registers a thread) plus its A fragments needs more than the 168 registers a thread
+  // that 384 threads leave: the producer warpgroup hands most of its registers to the consumers
+  constexpr bool REALLOC = MT * BN >= 256;
+  if (warp >= WG_CWARPS) {
+    if (REALLOC) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == WG_CWARPS && lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x.m[p.amap[tap]]) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_dy.m[p.bmap[tap]]) : "memory");
       const CUtensorMap* mb = &tm_dy.m[p.bmap[tap]];
@@ -156,43 +195,62 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   }
 
   // ===== consumer warpgroups =====
-  // k-block kb: transpose stage kb into buffer kb & 1 while this warpgroup's MMAs of kb - 1 (on the other buffer) run,
-  // then wait for those MMAs, then one CTA barrier, then issue the MMAs of kb.  Invariant: a warpgroup writes buffer
-  // kb & 1 only after the barrier of kb - 1, which both warpgroups reach only once their MMAs of kb - 2 (the last reads
-  // of that buffer) have retired; and the MMAs of kb start only after the barrier of kb, when both warpgroups' halves of
-  // the transposed tiles are written and made visible to the async proxy.
+  if (REALLOC) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  // The MT x 4 MMAs of a k-block (unit i / 4, k-step i % 4) go out in two commit groups of GK, each fed by its own A
+  // fragment registers.  k-block kb:
+  //   wait for G0 of kb - 1 (G1 of kb - 1 still runs) | load G0's fragments of kb | wait until dY buffer kb & 1 is free |
+  //   transpose the stage's dY into it | CTA barrier (both halves of the dY tile written and visible to the async proxy) |
+  //   issue G0 of kb | wait for G1 of kb - 1 (G0 of kb runs), which frees buffer (kb - 1) & 1 | load G1's fragments of
+  //   kb | release the stage | issue G1 of kb.
+  // Fragment registers are rewritten only once the MMAs that read them have retired; a dY buffer only once both
+  // warpgroups' MMAs of two k-blocks back have (buf_free: one arrive per consumer warp).  Each accumulator receives its
+  // MMAs in unit-major, k-step order, k-block after k-block.
+  constexpr int GK = 2 * MT;
   const int wg = warp >> 2;
+  const int cib = wg_a_channel(warp, lane), q = lane & 3;
+  const uint32_t a_box = (2 * wg + ((warp >> 1) & 1)) * WG_BOX + (cib & 3) * 4;
+  const uint32_t a_lo = a_box + q * 128 + ((((cib >> 2) ^ q) & 7) << 4);                // pixel 8k + q
+  const uint32_t a_hi = a_box + (q + 4) * 128 + ((((cib >> 2) ^ (q + 4)) & 7) << 4);    // pixel 8k + q + 4
+  const bool all_units = MT == 1 || nu == MT;   // uniform over the CTA: the last tile of an odd unit count has one
   float acc[MT][BN / 2];
 #pragma unroll
   for (int u = 0; u < MT; ++u)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[u][i] = 0.f;
+  uint32_t fa[2][GK][4];
   int stage = 0;
   uint32_t phase = 0;
   for (int kb = 0; kb < num_kb; ++kb) {
+    const int h = kb & 1;
     mbar_wait(&full_bar[stage], phase);
     const uint32_t s_addr = smem_u32(smem + stage * stage_bytes);
-    const uint32_t t_addr = smem_u32(tbuf + (kb & 1) * stage_bytes);
-    for (int i = 0; i < nu; ++i) wg_transpose<128>(t_addr + i * WG_A_BYTES, s_addr + i * WG_A_BYTES, p.round_a, warp, lane);
-    wg_transpose<BN>(t_addr + a_bytes, s_addr + a_bytes, p.round_b, warp, lane);
-    // the warp's reads of the TMA stage are complete (their values are stored): release it to the producer
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    const uint32_t t_addr = smem_u32(tbuf + h * b_bytes);
+    wgmma_wait<1>();                              // G0 of kb - 1 retired
+    wg_load_a<GK>(fa[0], s_addr, a_lo, a_hi, p.round_a);
+    if (kb >= 2) mbar_wait(&buf_free[h], ((kb >> 1) & 1) ^ 1);
+    wg_transpose<BN>(t_addr, s_addr + a_bytes, p.round_b, warp, lane);
     fence_proxy_async();
-    wgmma_wait<0>();                              // this warpgroup's MMAs of kb - 1 retired
     named_bar(1, 32 * WG_CWARPS);
 #pragma unroll
     for (int u = 0; u < MT; ++u)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
     wgmma_fence();
-    // all MT units (one past the end multiplies stale rows that are never stored): one unconditional chain of MMAs
 #pragma unroll
-    for (int u = 0; u < MT; ++u) {
+    for (int e = 0; e < GK; ++e)                  // 8 pixels (32 B of every dY row) per MMA
+      wgmma_tf32_rs<BN>(acc[e / 4], fa[0][e], make_desc(t_addr + (e % 4) * 32));
+    wgmma_commit();
+    wgmma_wait<1>();                              // G1 of kb - 1 retired: its dY buffer is free
+    if (kb >= 1 && lane == 0) mbar_arrive(&buf_free[h ^ 1]);
+    if (all_units) wg_load_a<GK>(fa[1], s_addr + (GK / 4) * WG_A_BYTES + (GK % 4) * 1024, a_lo, a_hi, p.round_a);
+    // the warp's reads of the TMA stage are complete (fragments loaded, dY values stored): release it to the producer
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    wgmma_fence();
+    if (all_units) {                              // a CTA past the last unit issues no MMAs for it
 #pragma unroll
-      for (int k = 0; k < WG_P / 8; ++k)          // 8 pixels (32 B of every row) per MMA
-        wgmma_tf32<BN>(acc[u], make_desc(t_addr + u * WG_A_BYTES + wg * (WG_A_BYTES / 2) + k * 32),
-                       make_desc(t_addr + a_bytes + k * 32));
+      for (int e = 0; e < GK; ++e)
+        wgmma_tf32_rs<BN>(acc[(GK + e) / 4], fa[1][e], make_desc(t_addr + ((GK + e) % 4) * 32));
     }
     wgmma_commit();
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -202,7 +260,8 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
   for (int u = 0; u < MT; ++u)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc_fence(acc[u][i]);
-  // epilogue: rows ci = m, m + 8 of each unit's tile, columns co0 + 8j + 2 (lane % 4) + {0, 1}
+  // epilogue: accumulator rows lane / 4 and lane / 4 + 8 are channels ci = cib, cib + 1 of the thread's box (see
+  // wg_a_channel), columns co0 + 8j + 2 (lane % 4) + {0, 1}
   const int c2 = (lane & 3) * 2;
   const bool vec2 = (p.cout & 1) == 0;
 #pragma unroll
@@ -211,7 +270,7 @@ wgrad_tc_kernel(const __grid_constant__ BMaps tm_x, const __grid_constant__ BMap
     const int uu = u0 + u, utap = uu / p.ci_tiles, ci0 = (uu % p.ci_tiles) * 128;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
+      const int row = (2 * wg + ((warp >> 1) & 1)) * 32 + cib + h;
       if (ci0 + row >= p.cin) continue;          // the last ci tile may hang over Cin (TMA zero-filled those channels)
       float* orow = p.partial + (((long long)split * p.taps_total + p.wtap[utap]) * p.cin + ci0 + row) * p.cout + co0;
 #pragma unroll
@@ -273,15 +332,15 @@ int pick_bn(int ncols) {
   return 0;
 }
 
-// TMA ring depth for a shared-memory budget (ring + the two transposed buffers; the barrier placement in the consumer
-// loop lets the transpose overlap the MMAs without a third one); returns the dynamic smem size.  A 48 KB stage (BN 256
-// with MT 1, or BN 128 with MT 2) gets a 2-deep ring and one CTA per SM; stages up to 24 KB fit two CTAs per SM.
-size_t wg_smem(size_t stage_bytes, size_t budget, int* stages) {
-  long long s = (long long)(budget / stage_bytes) - 2;
+// TMA ring depth for a shared-memory budget (ring + the two transposed dY tiles; the barrier placement in the consumer
+// loop lets the transpose overlap the MMAs without a third one); returns the dynamic smem size.  At one CTA per SM a
+// 48 KB stage (BN 256 with MT 1, or BN 128 with MT 2) gets a 3- or 4-deep ring.
+size_t wg_smem(size_t stage_bytes, size_t t_bytes, size_t budget, int* stages) {
+  long long s = ((long long)budget - 2 * (long long)t_bytes) / (long long)stage_bytes;
   if (s > WG_MAX_STAGES) s = WG_MAX_STAGES;
   if (s < 2) s = 2;
   *stages = (int)s;
-  return (size_t)(s + 2) * stage_bytes + 1024 + 256;
+  return (size_t)s * stage_bytes + 2 * t_bytes + 1024 + 256;
 }
 
 template <int BN, int MT, bool PART>
@@ -348,7 +407,8 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
   bool same_b = true;
   for (int i = 1; i < t.ntaps; ++i) same_b = same_b && p.bmap[i] == p.bmap[0];
   p.mt = (!g.per_image && ctx->tc_mt_max >= 2 && same_b && units >= 2 && 2 * p.bn <= WG_ACC_COLS) ? 2 : 1;
-  const size_t stage_bytes = (size_t)p.mt * WG_A_BYTES + (size_t)(p.bn / 32) * WG_BOX;
+  const size_t t_bytes = (size_t)(p.bn / 32) * WG_BOX;
+  const size_t stage_bytes = (size_t)p.mt * WG_A_BYTES + t_bytes;
   const long long tiles = (long long)p.co_tiles * ((units + p.mt - 1) / p.mt);
   int splits;
   size_t smem;
@@ -356,9 +416,10 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
     // "split" i = image i: its partial tile IS the result dw[i]
     p.kb_per_split = gh * gw / WG_P;
     splits = n;
-    smem = wg_smem(stage_bytes, 110 * 1024, &p.stages);
+    smem = wg_smem(stage_bytes, t_bytes, 110 * 1024, &p.stages);
   } else {
-    const bool two_ctas = wg_smem(stage_bytes, 110 * 1024, &p.stages) <= 113 * 1024;
+    // stages of up to 24 KB (BN <= 64 with MT 1) run two CTAs per SM
+    const bool two_ctas = stage_bytes <= 24 * 1024;
     // two CTAs per SM in total (two waves when only one fits), rounded DOWN so the grid never spills a few CTAs into an
     // extra wave; the pixel chain each fp32 accumulator sums stays as short as with two resident CTAs per SM
     splits = (int)((2ll * ctx->num_sms) / tiles);
@@ -367,7 +428,7 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
     if (splits < 1) splits = 1;
     p.kb_per_split = (p.kblocks + splits - 1) / splits;
     splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
-    smem = wg_smem(stage_bytes, two_ctas ? 110 * 1024 : 220 * 1024, &p.stages);
+    smem = wg_smem(stage_bytes, t_bytes, two_ctas ? 110 * 1024 : 225 * 1024, &p.stages);
   }
 
   const bool reduce = !g.per_image && splits > 1;
@@ -384,7 +445,7 @@ int cgan_wgrad_tc(cgan_ctx* ctx, const TcWgrad& g) {
   memset(&tm_x, 0, sizeof(tm_x));
   memset(&tm_dy, 0, sizeof(tm_dy));
   for (int v = 0; v < 4; ++v)
-    if (!make_view_map(&tm_x.m[v], g.x, v, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE) ||
+    if (!make_view_map(&tm_x.m[v], g.x, v, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_128B) ||
         !make_view_map(&tm_dy.m[v], g.dy, v, p.bw, p.bh, p.bni, CU_TENSOR_MAP_SWIZZLE_NONE))
       return cgan_fail(ctx, CGAN_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed%s", "cgan_wgrad_tc");
   int rc = wg_launch(ctx, dim3((unsigned)tiles, (unsigned)splits), smem, tm_x, tm_dy, p);
