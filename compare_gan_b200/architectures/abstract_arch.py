@@ -6,12 +6,17 @@ gin files bind `G.batch_norm_fn`, `G.spectral_norm`, `D.spectral_norm`, ... (ref
 """
 from .. import gin_lite as gin
 from .. import kernels as K
+from .. import tape
 from .. import utils
 from .. import variables as V
 
 
 class _Network(object):
   """What generators and discriminators share: a named variable scope and the configured normalisation."""
+
+  # cut a recomputed segment (tape.segment) per residual / non-local block; set by ModularGAN.build when the activation
+  # stash of a training update would not fit in device memory
+  recompute = False
 
   def _setup(self, name, batch_norm_fn, spectral_norm):
     self._name = name
@@ -33,7 +38,7 @@ class _Network(object):
     if state is None or state[0]() is not store:
       import weakref
       state = states[id(store)] = (weakref.ref(store), K.SNBatch())
-    with K.sn_batch(state[1]), V.variable_scope(self._name):
+    with K.sn_batch(state[1]), V.variable_scope(self._name), tape.segments(self.recompute):
       return self.apply(**inputs)
 
   def batch_norm(self, inputs, **kwargs):

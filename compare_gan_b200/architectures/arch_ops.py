@@ -8,22 +8,36 @@ import numpy as np
 
 from .. import gin_lite as gin
 from .. import kernels as K
+from .. import tape
 from .. import variables as V
 from ..gans import consts
 from ..tpu import tpu_ops
 
 
 # test hook: callables fn(scope_name, tensor) receiving the output of every linear / un-fused conv2d / deconv2d /
-# non_local_block / residual block, keyed by the variable scope it ran in (the oracle has the same hook)
+# non_local_block / residual block, keyed by the variable scope it ran in (the oracle has the same hook); once per forward,
+# not again when a recomputed segment replays it
 ACT_OBSERVERS = []
 
 
 def observe(y, suffix=None):
-  if ACT_OBSERVERS:
+  if ACT_OBSERVERS and not tape.replaying():
     name = "/".join(V.current()._scope + ([suffix] if suffix else []))
     for fn in ACT_OBSERVERS:
       fn(name, y)
   return y
+
+
+def recomputed(fn, *inputs):
+  """fn(*inputs) as one recomputed segment of the tape (tape.segment; a residual or non-local block, when the network
+  recomputes its blocks): its backward replays fn in the variable store and scope of the first pass."""
+  store = V.current()
+  scope = list(store._scope)
+
+  def run(*xs):
+    with V.use(store), store.at_scope(scope):
+      return fn(*xs)
+  return tape.segment(run, list(inputs))
 
 
 # ----------------------------------------------------------------------------- initializers
@@ -304,7 +318,11 @@ def lrelu(inputs, leak=0.2, name="lrelu", _tf32=False):
 
 
 def non_local_block(x, name, use_sn):
-  """Self-attention (non-local) block (reference arch_ops.py:709-758)."""
+  """Self-attention (non-local) block (reference arch_ops.py:709-758); one recomputed segment."""
+  return recomputed(lambda x_: _non_local_block(x_, name, use_sn), x)
+
+
+def _non_local_block(x, name, use_sn):
   with V.variable_scope(name):
     n, h, w, num_channels = x.shape
     num_channels_attn = num_channels // 8

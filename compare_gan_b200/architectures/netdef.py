@@ -121,6 +121,12 @@ def _norm_relu(batch_norm, layer_norm, x, idx, tf32, norm_kw):
 
 
 def residual_block(inputs, plan, batch_norm, z, y, is_training, use_sn, layer_norm=False):
+  """One recomputed segment (arch_ops.recomputed) of inputs, z and y: see _residual_block."""
+  return ops.recomputed(lambda x, z_, y_: _residual_block(x, plan, batch_norm, z_, y_, is_training, use_sn, layer_norm),
+                        inputs, z, y)
+
+
+def _residual_block(inputs, plan, batch_norm, z, y, is_training, use_sn, layer_norm):
   """norm-relu-conv, norm-relu-conv plus the plan's shortcut.  A generator block resamples in its FIRST convolution, a
   discriminator block in its SECOND (reference resnet_ops.py:93-102).  `layer_norm` puts ln1 / ln2 behind bn1 / bn2
   (the `D.layer_norm` binding).

@@ -63,6 +63,10 @@ class BigGanDeepResNetBlock(object):
       return skip
 
   def apply(self, inputs, z, y, is_training):
+    """One recomputed segment (arch_ops.recomputed) of inputs, z and y."""
+    return ops.recomputed(lambda x, z_, y_: self._apply(x, z_, y_, is_training), inputs, z, y)
+
+  def _apply(self, inputs, z, y, is_training):
     if _channels(inputs) != self._in_channels:
       raise ValueError("Unexpected number of input channels (expected {}, got {}).".format(
           self._in_channels, _channels(inputs)))

@@ -34,6 +34,20 @@ class AdamOptimizer(object):
 gin.external_configurable(AdamOptimizer, "tf.train.AdamOptimizer")
 
 
+HEADROOM_BYTES = 12 << 30
+
+
+def memory_budget():
+  """Device bytes the activation stash of a training update may take: what the device and torch's allocator cache hold
+  free when the model is built, less HEADROOM_BYTES for the backward pass's working tensors (a recomputed block's replay
+  among them) and the allocator's fragmentation.  None without a CUDA device (the CPU emulator of the C-ABI).  Tests
+  replace this function to force recomputation."""
+  if K._RT["device"].type != "cuda":
+    return None
+  free, _ = torch.cuda.mem_get_info()
+  return free + torch.cuda.memory_reserved() - torch.cuda.memory_allocated() - HEADROOM_BYTES
+
+
 class _FlatAdam(object):
   def __init__(self, opt, flat):
     self.opt, self.flat = opt, flat
@@ -89,6 +103,7 @@ class ModularGAN(AbstractGAN):
     self._graph = None
     self._built_batch = None
     self.d_kernels = None            # K.KernelSegments of D's kernels when the bound penalty is l2_penalty
+    self.recompute = {"generator": False, "discriminator": False}     # per network: blocks recomputed (see build)
 
   # ---- architecture registry (reference :169-213) ---------------------------------------------
   @property
@@ -184,9 +199,63 @@ class ModularGAN(AbstractGAN):
     self.ema = None
     if self._g_use_ema:
       self.ema = tape.DT(self.flat_g["param"].t.clone())
+    self.recompute = self._choose_recompute(b)
+    self.generator.recompute = self.recompute["generator"]
+    self.discriminator.recompute = self.recompute["discriminator"]
     self._built_batch = b
     torch.cuda.synchronize()
     return self
+
+  def _choose_recompute(self, b):
+    """Which networks recompute their blocks in the backward pass (tape.segment) instead of stashing their activations.
+    The stash of each network, plain and segmented, is measured after one recorded forward at 1 and at 2 images per
+    replica and extrapolated linearly to the built batch (B images for G, 2B for D); a D-update holds D's stash, a
+    G-update G's and D's.  The first choice among: nothing, the network with the larger stash, both, whose two updates
+    fit memory_budget() is taken.  A second-order gradient penalty differentiates through D twice, which a replay does
+    not support: such a model keeps the stash path, as does any model off the GPU unless the budget is forced."""
+    none = {"generator": False, "discriminator": False}
+    budget = memory_budget()
+    if budget is None or penalty_lib.bound_penalty() in (penalty_lib.wgangp_penalty, penalty_lib.dragan_penalty):
+      return none
+    at1, at2 = self._stash_bytes(1), self._stash_bytes(2)
+    self.store.reset_to_init()           # undo the measurement's BN / u_var updates
+    stash = {k: at1[k] + (at2[k] - at1[k]) * ((2 * b if k[0] == "discriminator" else b) - 1) for k in at1}
+    self.predicted_stash = dict(stash, budget=budget)          # (read by profiles/prof_biggan_batch256.py)
+
+    def fits(choice):
+      g, d = stash[("generator", choice["generator"])], stash[("discriminator", choice["discriminator"])]
+      return max(d, g + d) <= budget
+    larger = max(("generator", "discriminator"), key=lambda n: stash[(n, False)] - stash[(n, True)])
+    for choice in (none, dict(none, **{larger: True})):
+      if fits(choice):
+        return choice
+    return {"generator": True, "discriminator": True}
+
+  def _stash_bytes(self, n):
+    """{(network, segmented): device bytes one recorded forward at n images per replica keeps alive} (0 off the GPU)."""
+    out = {}
+    cuda = K._RT["device"].type == "cuda"
+    h, w, c = self._dataset.image_shape
+    dev = K._RT["device"]
+    z = tape.DT(torch.zeros(n, self._z_dim, device=dev))
+    images = tape.DT(torch.zeros(n, h, w, c, device=dev))
+    labels = tape.DT(torch.zeros(n, dtype=torch.int32, device=dev))
+    for name, net, x in (("generator", self.generator, z), ("discriminator", self.discriminator, images)):
+      for seg in (False, True):
+        out[(name, seg)] = 0
+        if not cuda:
+          continue
+        net.recompute = seg
+        torch.cuda.synchronize()
+        before = torch.cuda.memory_allocated()
+        with V.use(self.store), tape.record(True):
+          y = self._get_one_hot_labels(labels) if self.conditional else None
+          held = net(x, y=y, is_training=True)
+          torch.cuda.synchronize()
+          out[(name, seg)] = torch.cuda.memory_allocated() - before
+        del held, y
+        net.recompute = False
+    return out
 
   def _build_networks(self, f):
     """One dry generator / discriminator call that creates every variable (like TF graph construction)."""

@@ -17,7 +17,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .tape import DT, attach, no_record, recording
+from .tape import DT, attach, no_record, producers, recording, replayed, replaying
 from .tape import grad_accumulator as _grad_accumulator, take_sink as _take_sink, sole_consumer as _sole_consumer
 
 _RT = {"lib": None, "device": None, "math_mode": 0}
@@ -93,14 +93,11 @@ def _grad_feeds_tc(t):
   TF32-rounded and the contraction skips its rounding pass; a wrong guess only costs that pass.)"""
   if not tf32_on() or (t is not None and len(t.shape) == 4 and t.shape[-1] <= 4):
     return False          # (3-channel image-side contractions round their thin operand while gathering the patch tensor)
-  for _ in range(4):
-    if t is None or t.node is None:
-      return False
-    if t.node.name in _TC_NODES:
+  for name in producers(t, 4):
+    if name in _TC_NODES:
       return True
-    if t.node.name not in _PASS_NODES:
+    if name not in _PASS_NODES:
       return False
-    t = t.node.inputs[0]
   return False
 
 ACT_RELU, ACT_LRELU, ACT_SIGMOID, ACT_TANH01 = 1, 2, 3, 4
@@ -497,7 +494,7 @@ def conv2d(x, w, bias=None, stride=1, upsample=False, padding="SAME", relu=False
   if residual is not None and residual.shape != (d.n, d.oh, d.ow, d.cout):
     raise ValueError("conv2d: residual shape %s does not match the output %s" % (residual.shape, (d.n, d.oh, d.ow, d.cout)))
   y = _conv_fwd_raw(d, x, w, bias, relu, residual, round_out)
-  if relu and RELU_OBSERVERS:
+  if relu and RELU_OBSERVERS and not replaying():
     for fn in RELU_OBSERVERS:
       fn(y.t > 0)
   yv = DT(y.t) if relu else None        # y > 0  <=>  pre-activation > 0
@@ -744,12 +741,13 @@ def bias_add(x, bias):
 # ------------------------------------------------------------------------------------ pointwise / pooling
 
 RELU_OBSERVERS = []     # test hook: callables receiving the boolean "input > 0" mask of every (leaky-)ReLU evaluated
+                        # (once per forward: not again when a recomputed segment replays it, tape.segment)
 
 
 def act(x, kind, leak=0.0, round_tf32=False):
   """Pointwise activation; `round_tf32` (math_mode 1): the result only feeds tensor-core contractions, store it
   TF32-rounded so that they skip their operand-rounding pass."""
-  if RELU_OBSERVERS and kind in (ACT_RELU, ACT_LRELU):
+  if RELU_OBSERVERS and kind in (ACT_RELU, ACT_LRELU) and not replaying():
     for fn in RELU_OBSERVERS:
       fn(x.t > 0)
   y = empty(*x.shape)
@@ -1111,16 +1109,21 @@ def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_afte
   c = x.shape[-1]
   rows = x.numel // c
   rps = rows // x.shape[0]
-  stats = empty(2 * c)
-  _call("bn_moments", stats.ptr, x.ptr, rows, c)
-  if allreduce is not None and world > 1:
-    allreduce(stats)
-    _call("axpby", stats.ptr, 1.0 / world, stats.ptr, 0.0, None, 0.0, 2 * c)
-  mv = empty(2 * c)
-  mm = state.moving_mean if state is not None else None
-  mvv = state.moving_var if state is not None else None
-  _call("bn_finalize", mv.ptr, stats.ptr, c, None if mm is None else mm.ptr, None if mvv is None else mvv.ptr,
-        float(decay))
+
+  def moments():
+    """[2C] mean / variance of the (cross-replica) batch; updates the moving averages.  A segment's replay reuses them."""
+    stats = empty(2 * c)
+    _call("bn_moments", stats.ptr, x.ptr, rows, c)
+    if allreduce is not None and world > 1:
+      allreduce(stats)
+      _call("axpby", stats.ptr, 1.0 / world, stats.ptr, 0.0, None, 0.0, 2 * c)
+    mv = empty(2 * c)
+    mm = state.moving_mean if state is not None else None
+    mvv = state.moving_var if state is not None else None
+    _call("bn_finalize", mv.ptr, stats.ptr, c, None if mm is None else mm.ptr, None if mvv is None else mvv.ptr,
+          float(decay))
+    return mv
+  mv = replayed(moments)
   y = empty(*x.shape)
   rnd = bool(round_out) and tf32_on()
   _call("bn_apply", y.ptr, x.ptr, rows, c, rps, mv.ptr, float(eps), None if gamma is None else gamma.ptr,
@@ -1131,7 +1134,7 @@ def bn_train(x, gamma, beta, eps, state=None, decay=0.999, cond=False, relu_afte
   if relu_after:
     y.relu_of = (yv, 0.0)
   y_id = id(y)
-  if relu_after and RELU_OBSERVERS:
+  if relu_after and RELU_OBSERVERS and not replaying():
     for fn in RELU_OBSERVERS:
       fn(y.t > 0)
 
@@ -1223,7 +1226,7 @@ def self_modulation(z, wh, bh, wg, bg, wb, bb):
   h = empty(n, hidden) if hidden else None
   _call("self_modulation_fwd", gb.ptr, None if h is None else h.ptr, z.ptr, n, zd, hidden,
         None if wh is None else wh.ptr, None if bh is None else bh.ptr, wg.ptr, bg.ptr, wb.ptr, bb.ptr, c)
-  if h is not None and RELU_OBSERVERS:
+  if h is not None and RELU_OBSERVERS and not replaying():
     for fn in RELU_OBSERVERS:
       fn(h.t > 0)
   t, k = _tk(z)
@@ -1276,8 +1279,9 @@ def layer_norm(x, gamma, beta, relu_after=False, round_out=False):
   yv = DT(y.t) if relu_after else None
   if relu_after:
     y.relu_of = (yv, 0.0)
-    for fn in RELU_OBSERVERS:
-      fn(y.t > 0)
+    if not replaying():
+      for fn in RELU_OBSERVERS:
+        fn(y.t > 0)
   y_id = id(y)
 
   def vjp(g, needs):
@@ -1326,19 +1330,23 @@ def spectral_normalize(w, u, left, eps=1e-12):
   `sn_batch` scope the small weights of a network are served from ONE batched launch (see SNBatch)."""
   rows = w.numel // w.shape[-1]
   cols = w.shape[-1]
-  batch = _SN_SCOPE[-1]
-  if batch is not None:
-    hit = batch.lookup(w, u, left, eps)
-    if hit is not None:
-      wbar, v, sigma, u_used = hit
-      return _sn_attach(w, wbar, rows, cols, left, u_used, v, sigma)
-  v = empty(cols if left else rows)
-  sigma = empty(1)
-  wbar = empty(*w.shape)
-  _call("spectral_norm", w.ptr, rows, cols, int(left), float(eps), u.ptr, v.ptr, sigma.ptr, wbar.ptr)
-  # the backward needs u AFTER this call's update; later calls overwrite u_var, so keep a copy
-  u_used = empty(*u.shape)
-  _call("copy", u_used.ptr, u.ptr, u.numel)
+
+  def iterate():
+    """(wbar, v, sigma, u_used); advances u.  A segment's replay reuses them (u advances once per call site)."""
+    batch = _SN_SCOPE[-1]
+    if batch is not None:
+      hit = batch.lookup(w, u, left, eps)
+      if hit is not None:
+        return hit
+    v = empty(cols if left else rows)
+    sigma = empty(1)
+    wbar = empty(*w.shape)
+    _call("spectral_norm", w.ptr, rows, cols, int(left), float(eps), u.ptr, v.ptr, sigma.ptr, wbar.ptr)
+    # the backward needs u AFTER this call's update; later calls overwrite u_var, so keep a copy
+    u_used = empty(*u.shape)
+    _call("copy", u_used.ptr, u.ptr, u.numel)
+    return wbar, v, sigma, u_used
+  wbar, v, sigma, u_used = replayed(iterate)
   return _sn_attach(w, wbar, rows, cols, left, u_used, v, sigma)
 
 

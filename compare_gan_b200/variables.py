@@ -38,6 +38,15 @@ class VariableStore(object):
     finally:
       self._scope.pop()
 
+  @contextlib.contextmanager
+  def at_scope(self, scope):
+    """Runs the body in the scope path `scope` (a list of names), whatever scope is open."""
+    saved, self._scope = self._scope, list(scope)
+    try:
+      yield
+    finally:
+      self._scope = saved
+
   def full_name(self, name):
     return "/".join(self._scope + [name])
 
