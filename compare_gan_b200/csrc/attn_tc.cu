@@ -24,7 +24,17 @@
 // (V, K, dO or Q, transposed into [channel][row] tiles) therefore stores row 8s + r at k position r / 2 + 4 (r & 1).
 //
 // Operands are consumed as TF32: callers pass tensors already rounded to the nearest TF32 value (cgan_round_tf32 or a
-// producer's ROUND_OUT epilogue); P and dS are rounded to nearest here.  Accumulation is fp32.
+// producer's ROUND_OUT epilogue).  Accumulation is fp32.  Where the kernels round, per score (i, j) of image b:
+//   s  = Q_i . K_j (fp32 accumulation)     p = ex2.approx.ftz(s log2e - m_i log2e), m_i the row maximum (forward) or
+//                                              ex2.approx.ftz(s log2e - lse_i log2e) (both backward kernels)
+//   forward:  l_i = sum_j p (fp32, p UNROUNDED),  O_i = (sum_j rna_tf32(p) V_j) / l_i,  lse_i = m_i + log l_i
+//   backward: dS = rna_tf32(p (dP - D_i)) from the UNROUNDED p in both kernels, dQ = dS K, dK = dS^T Q,
+//             dV = rna_tf32(p)^T dO
+// so the normaliser is the one lse describes, and dQ and dK are contractions of the same dS.  tests/abi_emulator.py
+// (attention_tf32_model) is this contract in numpy.
+//
+// Memory: q, k, v and dout are read as float4 (16-byte aligned), out, dq, dk and dv stored and lse read as float2 (8-byte
+// aligned); the entry points refuse other pointers with CGAN_ERR_UNSUPPORTED before launching anything.
 #include "tc_common.cuh"
 
 namespace {
@@ -321,9 +331,9 @@ attn_bwd_dkv_kernel(const float* __restrict__ q, const float* __restrict__ k, co
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int col = 2 * (i >> 2) + (i & 1);
-      const float pr = rnd_tf32(ex2(fmaf(s[i], AT_LOG2E, -lb[col])));
-      dp[i] = rnd_tf32(pr * (dp[i] - dd[col]));            // dS^T
-      s[i] = pr;                                           // P^T
+      const float pr = ex2(fmaf(s[i], AT_LOG2E, -lb[col]));
+      dp[i] = rnd_tf32(pr * (dp[i] - dd[col]));            // dS^T, from the unrounded P as in attn_bwd_dq_kernel
+      s[i] = rnd_tf32(pr);                                 // P^T
     }
     fence_acc(dv); fence_acc(dk);
     wgmma_fence();
@@ -355,6 +365,8 @@ void fill_params(AtParams* p, int lq, int lk, int dk, int dv) {
 }
 
 inline int nv_pad(int dv) { return (dv + 31) / 32 * 32; }      // V / dO columns zero-padded to whole swizzle rows
+
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
 size_t fwd_smem(int nv) { return 1024 + AT_TQ * 128 + AT_TK * 128 + (size_t)AT_TK * nv * 4; }
 size_t dq_smem(int nv) { return 1024 + AT_TQ * 128 + (size_t)AT_TQ * nv * 4 + AT_TK * 128 + (size_t)AT_TK * nv * 4 + AT_TK * 128; }
@@ -393,6 +405,9 @@ int cgan_attention_fwd(cgan_ctx* ctx, const float* q, const float* k, const floa
   if (!cgan_attention_supported(ctx, batch, lq, lk, dk, dv))
     return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: needs math_mode 1, lq, lk multiples of 128, dk <= 32 (x4), dv <= 128 (x16)%s",
                      "cgan_attention_fwd");
+  if (!aligned(q, 16) || !aligned(k, 16) || !aligned(v, 16) || !aligned(out, 8) || !aligned(lse, 8))
+    return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: needs q, k, v 16-byte aligned and out, lse 8-byte aligned%s",
+                     "cgan_attention_fwd");
   AtParams p;
   fill_params(&p, lq, lk, dk, dv);
   p.out = out; p.out2 = lse;
@@ -419,6 +434,10 @@ int cgan_attention_bwd(cgan_ctx* ctx, const float* q, const float* k, const floa
   CGAN_REQUIRE(ctx, q && k && v && out && lse && dout && dq && dk_out && dv_out, "null pointer");
   if (!cgan_attention_supported(ctx, batch, lq, lk, dk, dv))
     return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED, "%s: unsupported shape or math mode%s", "cgan_attention_bwd");
+  if (!aligned(q, 16) || !aligned(k, 16) || !aligned(v, 16) || !aligned(dout, 16) || !aligned(lse, 8) || !aligned(dq, 8) ||
+      !aligned(dk_out, 8) || !aligned(dv_out, 8))
+    return cgan_fail(ctx, CGAN_ERR_UNSUPPORTED,
+                     "%s: needs q, k, v, dout 16-byte aligned and lse, dq, dk, dv 8-byte aligned%s", "cgan_attention_bwd");
   void* ws = nullptr;
   int rc = cgan_ws(ctx, (size_t)batch * lq * sizeof(float), &ws);
   if (rc) return rc;

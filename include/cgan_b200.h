@@ -159,7 +159,9 @@ int cgan_gemm_batched(cgan_ctx*, int trans_a, int trans_b, int m, int n, int k, 
  * pass tensors that already hold TF32-representable values (cgan_round_tf32, or a producer's ROUND_OUT epilogue).
  * cgan_attention_supported returns 1 when the fused kernels accept the shape in the current math mode (math_mode 1,
  * lq and lk multiples of 128, dk <= 32 and a multiple of 4, dv <= 128 and a multiple of 16), else 0 — callers then
- * compose cgan_gemm_batched / cgan_softmax_* as the reference does. */
+ * compose cgan_gemm_batched / cgan_softmax_* as the reference does.  The kernels read q, k, v and dout as float4 and store
+ * out, dq, dk, dv and read lse as float2: other pointers (legal 4-byte-aligned ones) return CGAN_ERR_UNSUPPORTED without
+ * launching. */
 int cgan_attention_supported(cgan_ctx*, int batch, int lq, int lk, int dk, int dv);
 int cgan_attention_fwd(cgan_ctx*, const float* q, const float* k, const float* v, float* out, float* lse, int batch, int lq,
                        int lk, int dk, int dv);

@@ -34,6 +34,43 @@ def rna_tf32(a):
   return ((a.view(np.uint32) + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
 
 
+LOG2E = np.float32(1.4426950408889634)
+
+
+def _ex2_ftz(x):
+  """ex2.approx.ftz.f32 as the correctly rounded 2^x, results below 2^-126 flushed to zero."""
+  y = np.exp2(x.astype(np.float64)).astype(np.float32)
+  y[y < np.float32(2.0 ** -126)] = 0
+  return y
+
+
+def _fma32(a, b, c):
+  """fmaf(a, b, c): a * b is exact in float64, the sum rounds once (twice at worst, far below the criteria's scale)."""
+  return (a.astype(np.float64) * np.float64(b) + np.asarray(c, np.float64)).astype(np.float32)
+
+
+def attention_tf32_model(q, k, v, dout=None, out=None, lse=None):
+  """The fused attention kernels' arithmetic (csrc/attn_tc.cu, header) on float32 [batch, rows, channels] arrays of
+  TF32 values.  Forward (dout None): returns (out, lse).  Backward: returns (dq, dk, dv) from the forward's out and lse.
+    p = ex2.approx.ftz(s log2e - m log2e) with m the row maximum (forward) or lse (backward), s = q k^T in fp32
+    forward:  l = sum of the UNROUNDED p,  out = (rna_tf32(p) v) / l,  lse = m + log l
+    backward: D = rowsum(dout * out),  dS = rna_tf32(p (dout v^T - D)),  dq = dS k,  dk = dS^T q,  dv = rna_tf32(p)^T dout
+  Summation orders are numpy's; the kernels' differ by fp32 accumulation only."""
+  q, k, v = (np.asarray(a, np.float32) for a in (q, k, v))
+  s = np.matmul(q, k.transpose(0, 2, 1))
+  if dout is None:
+    m = s.max(2, keepdims=True)
+    p = _ex2_ftz(_fma32(s, LOG2E, -(m * LOG2E)))
+    l = p.sum(2, keepdims=True, dtype=np.float32)
+    o = np.matmul(rna_tf32(p), v) * (np.float32(1.0) / l)
+    return o.astype(np.float32), (m + np.log(l))[:, :, 0].astype(np.float32)
+  dout, out, lse = np.asarray(dout, np.float32), np.asarray(out, np.float32), np.asarray(lse, np.float32)
+  p = _ex2_ftz(_fma32(s, LOG2E, -(lse * LOG2E)[:, :, None]))
+  d = (dout * out).sum(2, keepdims=True, dtype=np.float32)
+  ds = rna_tf32(p * (np.matmul(dout, v.transpose(0, 2, 1)) - d))
+  return (np.matmul(ds, k), np.matmul(ds.transpose(0, 2, 1), q), np.matmul(rna_tf32(p).transpose(0, 2, 1), dout))
+
+
 def _desc(ref):
   d = ref._obj            # ctypes.byref(ConvDesc)
   return d
@@ -79,8 +116,8 @@ class EmulatedLib(object):
     assert (key == 1 and value in (1, 2)) or (key == 3 and value in (0, 1, 2)) or (key == 6 and value in (0, 1))
 
   def call(self, name, *args):
-    self.launches += 1
     getattr(self, "cgan_" + name)(*args)
+    self.launches += 1                   # a refused call (CganError) launches nothing
 
   # ---- context / utilities ------------------------------------------------------------------
   def cgan_ctx_set_math_mode(self, mode):
@@ -505,35 +542,35 @@ class EmulatedLib(object):
   def cgan_round_tf32(self, y, x, n):
     f32(y, n)[:] = rna_tf32(f32(x, n))
 
+  @staticmethod
+  def _require_aligned(name, wide, narrow):
+    """The kernels' vector accesses: `wide` pointers are read as float4, `narrow` ones as float2."""
+    if any(int(p) % 16 for p in wide) or any(int(p) % 8 for p in narrow):
+      from compare_gan_b200 import _lib
+      what = {"attention_fwd": "q, k, v 16-byte aligned and out, lse 8-byte aligned",
+              "attention_bwd": "q, k, v, dout 16-byte aligned and lse, dq, dk, dv 8-byte aligned"}[name]
+      raise _lib.CganError("cgan_%s failed (4): cgan_%s: needs %s" % (name, name, what))
+
   def cgan_attention_fwd(self, q, k, v, out, lse, batch, lq, lk, dk, dv):
     assert self.attention_supported(batch, lq, lk, dk, dv)
+    self._require_aligned("attention_fwd", (q, k, v), (out, lse))
     self.last_path = 1
-    Q = f32(q, batch * lq * dk).reshape(batch, lq, dk)
-    Kk = f32(k, batch * lk * dk).reshape(batch, lk, dk)
-    Vv = f32(v, batch * lk * dv).reshape(batch, lk, dv)
-    s = np.einsum("bqd,bkd->bqk", Q, Kk).astype(np.float32)
-    m = s.max(2, keepdims=True)
-    pe = rna_tf32(np.exp(s - m).astype(np.float32))
-    l = pe.sum(2, keepdims=True, dtype=np.float32)
-    f32(out, batch * lq * dv).reshape(batch, lq, dv)[:] = np.einsum("bqk,bkd->bqd", pe, Vv) / l
-    f32(lse, batch * lq).reshape(batch, lq)[:] = (m + np.log(l))[:, :, 0]
+    o, l = attention_tf32_model(f32(q, batch * lq * dk).reshape(batch, lq, dk), f32(k, batch * lk * dk).reshape(batch, lk, dk),
+                                f32(v, batch * lk * dv).reshape(batch, lk, dv))
+    f32(out, batch * lq * dv).reshape(batch, lq, dv)[:] = o
+    f32(lse, batch * lq).reshape(batch, lq)[:] = l
 
   def cgan_attention_bwd(self, q, k, v, out, lse, dout, dq, dk_out, dv_out, batch, lq, lk, dk, dv):
     assert self.attention_supported(batch, lq, lk, dk, dv)
+    self._require_aligned("attention_bwd", (q, k, v, dout), (lse, dq, dk_out, dv_out))
     self.last_path = 1
-    Q = f32(q, batch * lq * dk).reshape(batch, lq, dk)
-    Kk = f32(k, batch * lk * dk).reshape(batch, lk, dk)
-    Vv = f32(v, batch * lk * dv).reshape(batch, lk, dv)
-    O = f32(out, batch * lq * dv).reshape(batch, lq, dv)
-    dO = f32(dout, batch * lq * dv).reshape(batch, lq, dv)
-    L = f32(lse, batch * lq).reshape(batch, lq, 1)
-    p = np.exp(np.einsum("bqd,bkd->bqk", Q, Kk).astype(np.float32) - L).astype(np.float32)
-    dsum = (dO * O).sum(2, keepdims=True, dtype=np.float32)
-    ds = rna_tf32(p * (np.einsum("bqd,bkd->bqk", dO, Vv).astype(np.float32) - dsum))
-    p = rna_tf32(p)
-    f32(dq, batch * lq * dk).reshape(batch, lq, dk)[:] = np.einsum("bqk,bkd->bqd", ds, Kk)
-    f32(dk_out, batch * lk * dk).reshape(batch, lk, dk)[:] = np.einsum("bqk,bqd->bkd", ds, Q)
-    f32(dv_out, batch * lk * dv).reshape(batch, lk, dv)[:] = np.einsum("bqk,bqd->bkd", p, dO)
+    gq, gk, gv = attention_tf32_model(
+        f32(q, batch * lq * dk).reshape(batch, lq, dk), f32(k, batch * lk * dk).reshape(batch, lk, dk),
+        f32(v, batch * lk * dv).reshape(batch, lk, dv), dout=f32(dout, batch * lq * dv).reshape(batch, lq, dv),
+        out=f32(out, batch * lq * dv).reshape(batch, lq, dv), lse=f32(lse, batch * lq).reshape(batch, lq))
+    f32(dq, batch * lq * dk).reshape(batch, lq, dk)[:] = gq
+    f32(dk_out, batch * lk * dk).reshape(batch, lk, dk)[:] = gk
+    f32(dv_out, batch * lk * dv).reshape(batch, lk, dv)[:] = gv
 
   def cgan_rowdot(self, out, a, b, rows, cols):
     f32(out, rows)[:] = (f32(a, rows * cols).reshape(rows, cols).astype(np.float64) *

@@ -18,6 +18,7 @@ import torch
 
 from oracle import nets as onets
 from oracle import tf_ops as T
+from tests.abi_emulator import attention_tf32_model
 from tests.gpu_util import ReluSigns, assert_close, compare_grads, make_inputs, make_pair, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -168,24 +169,18 @@ class _InSitu(object):
     K = self.K
     t = lambda dt: torch.from_numpy(dt.cpu().copy())
     if kind in ("attention", "attention_bwd"):
-      # the fused kernels' arithmetic on the engine's own (TF32-rounded) operands: fp32 scores, probabilities and dS rounded
-      # to TF32 before their second contraction, everything else fp32
+      # the fused kernels' arithmetic (tests/abi_emulator.py attention_tf32_model) on the engine's own TF32 operands
       q, k, v = t(kw["q"]), t(kw["k"]), t(kw["v"])
-      s = torch.bmm(q, k.transpose(1, 2))
       if kind == "attention":
-        m = s.max(-1, keepdim=True).values
-        pe = T.rna_tf32(torch.exp(s - m))
-        l = pe.sum(-1, keepdim=True)
-        pairs = [("out", kw["out"], torch.bmm(pe, v) / l), ("lse", kw["lse"], (m + torch.log(l))[..., 0])]
+        out, lse = attention_tf32_model(q.numpy(), k.numpy(), v.numpy())
+        pairs = [("out", kw["out"], out), ("lse", kw["lse"], lse)]
       else:
-        o, lse, do = t(kw["out"]), t(kw["lse"]), t(kw["dout"])
-        pr = torch.exp(s - lse[..., None])
-        ds = T.rna_tf32(pr * (torch.bmm(do, v.transpose(1, 2)) - (do * o).sum(-1, keepdim=True)))
-        pairs = [("dq", kw["dq"], torch.bmm(ds, k)), ("dk", kw["dk"], torch.bmm(ds.transpose(1, 2), q)),
-                 ("dv", kw["dv"], torch.bmm(T.rna_tf32(pr).transpose(1, 2), do))]
+        dq, dk, dv = attention_tf32_model(q.numpy(), k.numpy(), v.numpy(), dout=t(kw["dout"]).numpy(),
+                                          out=t(kw["out"]).numpy(), lse=t(kw["lse"]).numpy())
+        pairs = [("dq", kw["dq"], dq), ("dk", kw["dk"], dk), ("dv", kw["dv"], dv)]
       for what, got, ref in pairs:
-        scale = float(np.linalg.norm(ref.numpy().ravel()))
-        err = float(np.linalg.norm((got.cpu() - ref.numpy()).ravel())) / max(scale, 1e-30)
+        scale = float(np.linalg.norm(ref.ravel()))
+        err = float(np.linalg.norm((got.cpu() - ref).ravel())) / max(scale, 1e-30)
         self.results.append((err, "%s %s%s" % (kind, what, tuple(q.shape) + tuple(v.shape[1:])), "tcgen05_tf32", scale))
       return
     if kind == "bmm":
