@@ -93,6 +93,15 @@ __device__ __forceinline__ float rna_tf32(float x) {
   return __uint_as_float(u);
 }
 
+// the (leaky-)ReLU backward gate, TF's rule: with leak != 0 (leaky ReLU, tf.maximum(x, leak x), whose gradient goes to
+// x on ties) v passes where x >= 0, -0 included; with leak 0 (ReLU, ReluGrad) where x > 0.  Elsewhere v is scaled by
+// leak.  x: the activation's input or output (same sign).  Both rules are one comparison x > relu_gate_threshold(leak):
+// x >= 0 is x > -2^-149, the negative float nearest to zero (the library is built without flush-to-zero).
+__host__ __device__ __forceinline__ float relu_gate_threshold(float leak) { return leak != 0.f ? -0x1p-149f : 0.f; }
+__device__ __forceinline__ float relu_gate(float x, float v, float leak) {
+  return x > relu_gate_threshold(leak) ? v : leak * v;
+}
+
 // element i of the counter-based uniform [0, 1) stream (cgan_random_uniform): SplitMix64 of (seed, i + 1), 24 mantissa bits
 __device__ __forceinline__ float splitmix_uniform(unsigned long long seed, unsigned long long i) {
   unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (i + 1ull);
@@ -224,7 +233,7 @@ struct TcConv {
   long long s_n, s_h, s_w, base;
   long long ph_base[4];
   int ph_h[4], ph_w[4];               // > 0: phase ph stores only rows < ph_h[ph], columns < ph_w[ph] (0: the whole grid)
-  // epilogue: + bias[col] + residual, then ReLU or the (leaky-)ReLU backward gate out = mask > 0 ? v : mask_leak * v,
+  // epilogue: + bias[col] + residual, then ReLU or the (leaky-)ReLU backward gate out = relu_gate(mask, v, mask_leak),
   // then TF32 rounding of the stored value
   const float* bias;
   const float* residual;

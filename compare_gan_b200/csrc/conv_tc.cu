@@ -50,7 +50,8 @@ struct TcParams {
   int vec2;                         // 1: every output row starts at an even element offset and cout is even (float2 stores)
   int round_a;                      // 1: round the activation tiles to nearest TF32 in shared memory (operand not pre-rounded)
   int round_out;                    // 1: store TF32-rounded outputs (the consumer is another tensor-core contraction)
-  float mask_leak;                  // with `mask`: out = ref > 0 ? v : mask_leak * v  ((leaky-)ReLU backward fused into a dgrad)
+  float mask_leak;                  // with `mask`: out = ref > mask_thr ? v : mask_leak * v  ((leaky-)ReLU backward fused into a dgrad)
+  float mask_thr;                   // relu_gate_threshold(mask_leak): relu_gate with the threshold chosen once on the host
   const float* residual;            // optional tensor of the output's geometry added before the activation (residual blocks)
   const float* mask;                // optional tensor of the output's geometry: the (leaky-)ReLU input/output whose sign gates v
   int wimg_stride;                  // batched GEMM: weight slice = wtap + image * wimg_stride (tiles never span images)
@@ -96,7 +97,7 @@ __device__ __forceinline__ float epilogue_one(const TcParams& p, float v, int co
   if (p.bias) v += p.bias[col];
   if (p.residual) v += p.residual[off];
   if (p.relu) v = fmaxf(v, 0.f);
-  if (p.mask) v = p.mask[off] > 0.f ? v : p.mask_leak * v;
+  if (p.mask) v = p.mask[off] > p.mask_thr ? v : p.mask_leak * v;
   if (p.round_out) v = rna_tf32(v);
   return v;
 }
@@ -131,7 +132,7 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float* ac
         if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
         if (p.mask) {
           const float2 mv = *reinterpret_cast<const float2*>(p.mask + off);
-          v.x = mv.x > 0.f ? v.x : p.mask_leak * v.x; v.y = mv.y > 0.f ? v.y : p.mask_leak * v.y;
+          v.x = mv.x > p.mask_thr ? v.x : p.mask_leak * v.x; v.y = mv.y > p.mask_thr ? v.y : p.mask_leak * v.y;
         }
         if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
         *reinterpret_cast<float2*>(p.out + off) = v;
@@ -179,7 +180,7 @@ __device__ __forceinline__ void tile_epilogue_smem(const TcParams& p, const CUte
         if (p.bias) { v.x += b.x; v.y += b.y; }
         if (p.residual) { v.x += e.x; v.y += e.y; }
         if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
-        if (p.mask) { v.x = e.x > 0.f ? v.x : p.mask_leak * v.x; v.y = e.y > 0.f ? v.y : p.mask_leak * v.y; }
+        if (p.mask) { v.x = e.x > p.mask_thr ? v.x : p.mask_leak * v.x; v.y = e.y > p.mask_thr ? v.y : p.mask_leak * v.y; }
         if (p.round_out) { v.x = rna_tf32(v.x); v.y = rna_tf32(v.y); }
         sts64(a, v);
       }
@@ -695,6 +696,7 @@ int cgan_conv_tc(cgan_ctx* ctx, const TcConv& c) {
   p.relu = c.relu;
   p.round_a = c.a.tf32 ? 0 : 1;
   p.round_out = c.round_out; p.residual = c.residual; p.mask = c.mask; p.mask_leak = c.mask_leak;
+  p.mask_thr = relu_gate_threshold(c.mask_leak);
   p.nphases = 1;
   p.ph_tap0[0] = 0; p.ph_tap0[1] = ntaps;
   p.ph_base[0] = c.base;

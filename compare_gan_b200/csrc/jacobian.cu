@@ -38,7 +38,7 @@ __device__ __forceinline__ long long primal_index(long long i, long long per, in
 
 __device__ __forceinline__ float act_deriv(float r, int kind, float leak) {
   if (kind == CGAN_ACT_RELU) return r > 0.f ? 1.f : 0.f;
-  if (kind == CGAN_ACT_LRELU) return r > 0.f ? 1.f : leak;
+  if (kind == CGAN_ACT_LRELU) return relu_gate(r, 1.f, leak);   // as act_bwd: ties (x = +-0) go to x
   if (kind == CGAN_ACT_SIGMOID) return r * (1.0f - r);
   const float t = 2.0f * r - 1.0f;       // y = (tanh + 1) / 2  ->  tanh = 2y - 1
   return 0.5f * (1.0f - t * t);

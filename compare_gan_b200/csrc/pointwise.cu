@@ -188,7 +188,7 @@ __device__ __forceinline__ float act_fwd_1(float v, int kind, float leak) {
 }
 __device__ __forceinline__ float act_bwd_1(float g, float r, int kind, float leak) {
   if (kind == CGAN_ACT_RELU) return r > 0.f ? g : 0.f;
-  if (kind == CGAN_ACT_LRELU) return (r > leak * r) ? g : ((r < leak * r) ? leak * g : 0.5f * (1.0f + leak) * g);
+  if (kind == CGAN_ACT_LRELU) return relu_gate(r, g, leak);     // tf.maximum(x, leak x): ties (x = +-0) go to x
   if (kind == CGAN_ACT_SIGMOID) return g * r * (1.0f - r);
   float t = 2.0f * r - 1.0f;       // y=(tanh+1)/2 -> tanh = 2y-1
   return g * 0.5f * (1.0f - t * t);
@@ -238,7 +238,7 @@ __global__ void conv_post_kernel(float* __restrict__ y, long long rows, int c, i
     float v = y[o];
     if (residual) v += residual[o];
     if (relu) v = fmaxf(v, 0.f);
-    if (mask) v = mask[o] > 0.f ? v : leak * v;
+    if (mask) v = relu_gate(mask[o], v, leak);
     if (round_out) v = rna_tf32(v);
     y[o] = v;
   }
@@ -486,7 +486,8 @@ __global__ void pool2d_fwd_v4_kernel(float4* __restrict__ y, const float4* __res
         ++cnt;
       }
     }
-    if (mode != 0) { float inv = 1.0f / (float)max(cnt, 1); acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv; }
+    // the correctly rounded quotient, as the scalar kernel: a product with 1 / cnt differs in the last bit for cnt 6, 9
+    if (mode != 0) { const float fc = (float)max(cnt, 1); acc.x /= fc; acc.y /= fc; acc.z /= fc; acc.w /= fc; }
     y[i] = acc;
   }
 }

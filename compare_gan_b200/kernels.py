@@ -520,8 +520,8 @@ def conv2d(x, w, bias=None, stride=1, upsample=False, padding="SAME", relu=False
 
 def conv2d_dgrad(d, dy, w, bias=None, round_out=False, relu_mask=None, mask_for=None):
   """Input gradient of conv2d == tf.nn.conv2d_transpose (+ bias, arch_ops.py:588-592).  `relu_mask` = (ref, leak): the
-  result is the gradient w.r.t. a (leaky-)ReLU output `mask_for`; that ReLU's backward (g * [ref > 0 ? 1 : leak]) is applied
-  in this kernel's epilogue and the result is tagged so the ReLU's own vjp passes it through."""
+  result is the gradient w.r.t. a (leaky-)ReLU output `mask_for`; that ReLU's backward (g where ref > 0, or ref >= 0 for a
+  leak != 0; g * leak elsewhere) is applied in this kernel's epilogue and the result is tagged so the ReLU's own vjp passes it through."""
   dx = empty(d.n, d.h, d.w, d.cin)
   rnd = bool(round_out) and tf32_on()
   mref, mleak = relu_mask if relu_mask is not None else (None, 0.0)

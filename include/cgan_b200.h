@@ -123,8 +123,9 @@ int cgan_conv2d_wgrad(cgan_ctx*, const cgan_conv_desc*, const float* x, const fl
  * inside its residual blocks is done in the convolution's epilogue, so each activation tensor crosses HBM once:
  *   y = act(conv(x, w) + bias + residual)                 residual add of resnet_ops.py:181 / resnet_biggan.py:150
  *   act = ReLU when flags & CGAN_CONV_RELU                 tf.nn.relu of resnet_ops.py:161,174 (the consumer's pre-activation)
- *   y = mask > 0 ? y : mask_leak * y                       the (leaky-)ReLU gradient (arch_ops.py:595-597) applied to an input
- *                                                          gradient: mask is the activation's input (or output), same shape as y
+ *   y = pass ? y : mask_leak * y                           the (leaky-)ReLU gradient (arch_ops.py:595-597) applied to an input
+ *                                                          gradient: mask is the activation's input (or output), same shape as y;
+ *                                                          pass = mask >= 0 (-0 included) for leaky ReLU, mask > 0 for ReLU
  *   CGAN_CONV_ROUND_OUT: y is stored rounded to the nearest TF32 value (its only consumers are tensor-core contractions,
  *   which would round it anyway); CGAN_CONV_IN_TF32 / CGAN_CONV_IN2_TF32 assert that the first / second activation operand
  *   (x or dy; for wgrad x and dy) already holds TF32-representable values, so the kernel skips its operand-rounding pass.
@@ -134,7 +135,7 @@ typedef struct {
   const float* bias;        /* [cout] (fwd) / [cin] (dgrad), nullable */
   const float* residual;    /* same shape as the output, nullable */
   const float* mask;        /* same shape as the output, nullable */
-  float mask_leak;          /* 0 for ReLU, the leak for leaky ReLU */
+  float mask_leak;          /* 0 for ReLU, the leak for leaky ReLU (a leak of 0 means ReLU) */
   int32_t flags;
   int32_t ldy;
 } cgan_conv_epilogue;
@@ -297,7 +298,8 @@ enum { CGAN_ACT_RELU = 1, CGAN_ACT_LRELU = 2, CGAN_ACT_SIGMOID = 3, CGAN_ACT_TAN
  * tensor only feeds tensor-core contractions, which then skip their own operand-rounding pass (math_mode 1 only). */
 enum { CGAN_ACT_ROUND_TF32 = 0x100 };
 int cgan_act_fwd(cgan_ctx*, float* y, const float* x, int kind, float leak, int64_t n);
-/* dx = dy * act'(.) ; `ref` is x for relu/lrelu and y for sigmoid/tanh01 */
+/* dx = dy * act'(.) ; `ref` is x for relu/lrelu and y for sigmoid/tanh01.  TF's rule at 0: relu' = [ref > 0] (ReluGrad),
+ * lrelu' = 1 where ref >= 0, -0 included (tf.maximum(x, leak x) sends a tie's gradient to x), else leak. */
 int cgan_act_bwd(cgan_ctx*, float* dx, const float* dy, const float* ref, int kind, float leak, int64_t n);
 int cgan_add(cgan_ctx*, float* y, const float* a, const float* b, int64_t n);
 /* same, optionally storing TF32-rounded sums (gradient accumulation in front of a tensor-core contraction) */
@@ -447,8 +449,8 @@ int cgan_fd_counts(cgan_ctx*, int64_t* counts, const double* dist, int64_t count
 /* ---- generator conditioning (metrics/jacobian_conditioning.py:32-173) ---- */
 /* Forward-mode tangents of the generator's nonlinear ops.  A tangent batch holds k tangents per primal sample,
  * sample-major: for n_primal samples of `per` values each, t[(s * k + j) * per + e] is tangent j of value e of sample s,
- * and the primal (ref / x / y / p) is read once per tangent: t_out = t_in * act'(ref), with ref = x for relu / lrelu (mask
- * ref > 0, else 0 / leak) and ref = y for sigmoid / tanh01, as cgan_act_bwd (arch_ops.py:595-597, sndcgan.py:74-78). */
+ * and the primal (ref / x / y / p) is read once per tangent: t_out = t_in * act'(ref), with ref = x for relu / lrelu (1 where
+ * ref > 0, else 0 / 1 where ref >= 0, else leak) and ref = y for sigmoid / tanh01, as cgan_act_bwd (arch_ops.py:595-597, sndcgan.py:74-78). */
 int cgan_act_jvp(cgan_ctx*, float* t_out, const float* t_in, const float* ref, int kind, float leak, int n_primal,
                  int64_t per, int k);
 /* Tangent of cgan_bn_apply with the moments constant (arch_ops.py:66-191, 423-445): r = rsqrt(var + eps),

@@ -20,6 +20,11 @@ def _check_pair(a, b):
     raise ValueError("Rank: expected 2, got %s and %s" % (len(a), len(b)))
 
 
+def _relu(x):
+  """tf.nn.relu with ReluGrad's gradient, 0 at the kink x = 0 (torch.clamp would pass 1 there)."""
+  return torch.where(x > 0, x, torch.zeros_like(x))
+
+
 def get_losses(fn, d_real, d_fake, d_real_logits, d_fake_logits):
   """gans/loss_lib.py:53-154 -> (d_loss, d_loss_real, d_loss_fake, g_loss)."""
   _check_pair(d_real_logits.shape, d_fake_logits.shape)
@@ -36,8 +41,8 @@ def get_losses(fn, d_real, d_fake, d_real_logits, d_fake_logits):
     lf = (d_fake ** 2).mean()
     return 0.5 * (lr + lf), lr, lf, 0.5 * ((d_fake - 1.0) ** 2).mean()
   if fn == "hinge":               # :127-148
-    lr = torch.clamp(1.0 - d_real_logits, min=0).mean()
-    lf = torch.clamp(1.0 + d_fake_logits, min=0).mean()
+    lr = _relu(1.0 - d_real_logits).mean()
+    lf = _relu(1.0 + d_fake_logits).mean()
     return lr + lf, lr, lf, -d_fake_logits.mean()
   raise ValueError(fn)
 

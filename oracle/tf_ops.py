@@ -234,8 +234,9 @@ def max_pool2(x):
 
 
 def lrelu(x, leak=0.2):
-  """arch_ops.py:595-597: max(x, leak*x)."""
-  return torch.maximum(x, leak * x)
+  """arch_ops.py:595-597: max(x, leak*x), with the gradient of TF's Maximum: 1 where x >= 0 (a tie, x = +-0, sends it to
+  x), leak elsewhere.  torch.maximum would split a tie's gradient between its arguments."""
+  return torch.where(x >= 0, x, leak * x)
 
 
 def l2_normalize(x, eps=1e-12):
@@ -294,9 +295,13 @@ def spectral_sigma(w2d, u, singular_value="left", eps=1e-12):
 
 
 def sigmoid_ce(logits, labels_one):
-  """tf.nn.sigmoid_cross_entropy_with_logits: max(x,0)-x*z+log1p(exp(-|x|))."""
+  """tf.nn.sigmoid_cross_entropy_with_logits: max(x,0)-x*z+log1p(exp(-|x|)), written as TF writes it (x >= 0 selects both
+  branches), so that its gradient is sigmoid(x) - z at x = 0 too (torch's clamp and abs would give 1 - z there)."""
   z = 1.0 if labels_one else 0.0
-  return torch.clamp(logits, min=0) - logits * z + torch.log1p(torch.exp(-logits.abs()))
+  pos = logits >= 0
+  relu_logits = torch.where(pos, logits, torch.zeros_like(logits))
+  neg_abs = torch.where(pos, -logits, logits)
+  return relu_logits - logits * z + torch.log1p(torch.exp(neg_abs))
 
 
 def orthogonal_init(rng, shape, gain=1.0):

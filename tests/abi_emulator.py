@@ -34,6 +34,39 @@ def rna_tf32(a):
   return ((a.view(np.uint32) + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
 
 
+def relu_pass(ref, leak):
+  """Where the (leaky-)ReLU backward passes the gradient unscaled, TF's rule, on a numpy array or a torch tensor: leaky
+  ReLU tf.maximum(x, leak x) where ref >= 0 (a tie, ref = +-0, sends the gradient to x); ReLU (leak 0) where ref > 0
+  (ReluGrad).  Elsewhere the gradient is scaled by leak (0 for ReLU).  ref: the activation's input or output."""
+  return ref >= 0 if leak != 0 else ref > 0
+
+
+def relu_mask(rng, shape):
+  """A (leaky-)ReLU input to gate with: standard normal, with exact +0 at every 5th and -0 at every 7th element, where
+  ReLU and leaky ReLU part ways."""
+  m = rng.standard_normal(shape).astype(np.float32)
+  m.ravel()[::5] = 0.0
+  m.ravel()[3::7] = -0.0
+  return m
+
+
+def relu_gate(ref, v, leak):
+  """The gradient v through the (leaky-)ReLU backward of relu_pass, rounded in v's own precision."""
+  return np.where(relu_pass(ref, leak), v, np.asarray(v).dtype.type(leak) * v)
+
+
+def act_deriv(r, kind, leak):
+  """act'(ref) of cgan_act_bwd / cgan_act_jvp in float32: ref = x for relu / lrelu, y for sigmoid / tanh01."""
+  if kind == 1:
+    return (r > 0).astype(np.float32)
+  if kind == 2:
+    return relu_gate(r, np.ones_like(r, np.float32), leak)
+  if kind == 3:
+    return r * (1 - r)
+  t = 2 * r - 1
+  return np.float32(0.5) * (1 - t * t)
+
+
 LOG2E = np.float32(1.4426950408889634)
 
 
@@ -161,8 +194,10 @@ class EmulatedLib(object):
 
   def cgan_scale_by_dev(self, y, x, scalar_dev, mul, inverse, n):
     s = f32(scalar_dev, 1)[0]
-    s = np.float32(1.0) / s if inverse else s
-    f32(y, n)[:] = f32(x, n) * (s * np.float32(mul))
+    if inverse and mul == 1.0:           # per element, as "w / norm_value" (arch_ops.py:531)
+      f32(y, n)[:] = f32(x, n) / s
+    else:
+      f32(y, n)[:] = f32(x, n) * (np.float32(mul) / s if inverse else np.float32(mul) * s)
 
   def cgan_dot(self, out_dev, a, b, n):
     f32(out_dev, 1)[0] = np.float32(np.dot(f32(a, n).astype(np.float64), f32(b, n).astype(np.float64)))
@@ -226,7 +261,7 @@ class EmulatedLib(object):
       np.maximum(o, 0, out=o)
     if ep.mask:
       m = f32(ep.mask, n)
-      o[:] = np.where(m > 0, o, np.float32(ep.mask_leak) * o)
+      o[:] = relu_gate(m, o, ep.mask_leak)
     if ep.flags & 2:
       o[:] = rna_tf32(o)
 
@@ -444,9 +479,9 @@ class EmulatedLib(object):
     rnd, kind = kind & 0x100, kind & 0xFF
     g, r = f32(dy, n), f32(ref, n)
     if kind == 1:
-      out = g * (r > 0)
+      out = np.where(r > 0, g, np.float32(0))
     elif kind == 2:
-      out = g * np.where(r > 0, np.float32(1.0), np.float32(leak))
+      out = relu_gate(r, g, leak)
     elif kind == 3:
       out = g * r * (1 - r)
     else:                                  # y = (tanh+1)/2  =>  dy/dx = (1 - tanh^2)/2 = 2 y (1 - y)
@@ -641,6 +676,48 @@ class EmulatedLib(object):
     a = f32(act, n * d).reshape(n, d).astype(np.float64)
     f64(s, d)[:] += a.sum(0)
     f64(sxx, d * d).reshape(d, d)[:] += a.T @ a
+
+  # ---- generator conditioning (csrc/jacobian.cu): k tangents per primal sample, sample-major ----------------------
+  def cgan_act_jvp(self, t_out, t_in, ref, kind, leak, n_primal, per, k):
+    r = f32(ref, n_primal * per).reshape(n_primal, 1, per)
+    t = f32(t_in, n_primal * k * per).reshape(n_primal, k, per)
+    f32(t_out, n_primal * k * per)[:] = (t * act_deriv(r, kind, leak)).ravel()
+
+  def cgan_bn_apply_jvp(self, t_y, t_x, x, y, rows, c, rps, mean_var, eps, gamma, t_gamma, t_beta, cond, k):
+    b = rows // rps
+    mv = f32(mean_var, 2 * c)
+    inv = np.float32(1.0) / np.sqrt(mv[c:] + np.float32(eps))
+    xv = f32(x, rows * c).reshape(b, 1, rps, c)
+    g = np.ones((1, 1, 1, c), np.float32)
+    if gamma is not None:
+      g = f32(gamma, (b if cond else 1) * c).reshape(-1, 1, 1, c)
+    out = np.zeros((b, k, rps, c), np.float32)
+    if t_x is not None:
+      out += f32(t_x, rows * k * c).reshape(b, k, rps, c) * inv * g
+    if t_gamma is not None:
+      out += (xv - mv[:c]) * inv * f32(t_gamma, b * k * c).reshape(b, k, 1, c)
+    if t_beta is not None:
+      out += f32(t_beta, b * k * c).reshape(b, k, 1, c)
+    if y is not None:
+      out *= f32(y, rows * c).reshape(b, 1, rps, c) > 0
+    f32(t_y, rows * k * c)[:] = out.ravel()
+
+  def cgan_maxpool2_jvp(self, t_out, t_in, x, n, h, w, c, k):
+    v = f32(x, n * h * w * c).reshape(n, h // 2, 2, w // 2, 2, c).transpose(0, 1, 3, 5, 2, 4).reshape(n, -1, 4)
+    arg = v.argmax(axis=2)                                   # the first maximum, as maxpool2_bwd
+    t = f32(t_in, n * k * h * w * c).reshape(n, k, h // 2, 2, w // 2, 2, c).transpose(0, 1, 2, 4, 6, 3, 5)
+    t = t.reshape(n, k, -1, 4)
+    out = np.take_along_axis(t, np.broadcast_to(arg[:, None, :, None], (n, k, arg.shape[1], 1)), axis=3)
+    f32(t_out, n * k * (h // 2) * (w // 2) * c)[:] = out.ravel()
+
+  def cgan_softmax_jvp(self, t_out, t_in, p, n, rps, cols, k):
+    pv = f32(p, n * rps * cols).reshape(n, 1, rps, cols).astype(np.float64)
+    t = f32(t_in, n * k * rps * cols).reshape(n, k, rps, cols).astype(np.float64)
+    f32(t_out, n * k * rps * cols)[:] = (pv * (t - (t * pv).sum(3, keepdims=True))).ravel()
+
+  def cgan_metric_tensor_f64(self, m, t, b, k, d):
+    tv = f32(t, b * k * d).reshape(b, k, d).astype(np.float64)
+    f64(m, b * k * k)[:] = np.matmul(tv, tv.transpose(0, 2, 1)).ravel()
 
 
 @contextlib.contextmanager

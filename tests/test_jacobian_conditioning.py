@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.abi_emulator import EmulatedLib, emulated_library, f32, f64
+from tests.abi_emulator import EmulatedLib, emulated_library
 
 
 def _jc():
@@ -14,67 +14,10 @@ def _jc():
   return jacobian_conditioning
 
 
-# ---- the new device entries, emulated on the CPU from their header contracts ----
+# ---- the device entries of csrc/jacobian.cu, emulated on the CPU from their header contracts (tests/abi_emulator.py) ----
 
-def _act_deriv(r, kind, leak):
-  if kind == 1:
-    return (r > 0).astype(np.float32)
-  if kind == 2:
-    return np.where(r > 0, np.float32(1.0), np.float32(leak))
-  if kind == 3:
-    return r * (1 - r)
-  t = 2 * r - 1
-  return np.float32(0.5) * (1 - t * t)
-
-
-def _emu_act_jvp(self, t_out, t_in, ref, kind, leak, n_primal, per, k):
-  r = f32(ref, n_primal * per).reshape(n_primal, 1, per)
-  t = f32(t_in, n_primal * k * per).reshape(n_primal, k, per)
-  f32(t_out, n_primal * k * per)[:] = (t * _act_deriv(r, kind, leak)).ravel()
-
-
-def _emu_bn_apply_jvp(self, t_y, t_x, x, y, rows, c, rps, mean_var, eps, gamma, t_gamma, t_beta, cond, k):
-  b = rows // rps
-  mv = f32(mean_var, 2 * c)
-  inv = np.float32(1.0) / np.sqrt(mv[c:] + np.float32(eps))
-  xv = f32(x, rows * c).reshape(b, 1, rps, c)
-  g = np.ones((1, 1, 1, c), np.float32)
-  if gamma is not None:
-    g = f32(gamma, (b if cond else 1) * c).reshape(-1, 1, 1, c)
-  out = np.zeros((b, k, rps, c), np.float32)
-  if t_x is not None:
-    out += f32(t_x, rows * k * c).reshape(b, k, rps, c) * inv * g
-  if t_gamma is not None:
-    out += (xv - mv[:c]) * inv * f32(t_gamma, b * k * c).reshape(b, k, 1, c)
-  if t_beta is not None:
-    out += f32(t_beta, b * k * c).reshape(b, k, 1, c)
-  if y is not None:
-    out *= f32(y, rows * c).reshape(b, 1, rps, c) > 0
-  f32(t_y, rows * k * c)[:] = out.ravel()
-
-
-def _emu_maxpool2_jvp(self, t_out, t_in, x, n, h, w, c, k):
-  v = f32(x, n * h * w * c).reshape(n, h // 2, 2, w // 2, 2, c).transpose(0, 1, 3, 5, 2, 4).reshape(n, -1, 4)
-  arg = v.argmax(axis=2)                                   # the first maximum, as maxpool2_bwd
-  t = f32(t_in, n * k * h * w * c).reshape(n, k, h // 2, 2, w // 2, 2, c).transpose(0, 1, 2, 4, 6, 3, 5)
-  t = t.reshape(n, k, -1, 4)
-  out = np.take_along_axis(t, np.broadcast_to(arg[:, None, :, None], (n, k, arg.shape[1], 1)), axis=3)
-  f32(t_out, n * k * (h // 2) * (w // 2) * c)[:] = out.ravel()
-
-
-def _emu_softmax_jvp(self, t_out, t_in, p, n, rps, cols, k):
-  pv = f32(p, n * rps * cols).reshape(n, 1, rps, cols).astype(np.float64)
-  t = f32(t_in, n * k * rps * cols).reshape(n, k, rps, cols).astype(np.float64)
-  f32(t_out, n * k * rps * cols)[:] = (pv * (t - (t * pv).sum(3, keepdims=True))).ravel()
-
-
-def _emu_metric_tensor_f64(self, m, t, b, k, d):
-  tv = f32(t, b * k * d).reshape(b, k, d).astype(np.float64)
-  f64(m, b * k * k)[:] = np.matmul(tv, tv.transpose(0, 2, 1)).ravel()
-
-
-_EMULATED = {"cgan_act_jvp": _emu_act_jvp, "cgan_bn_apply_jvp": _emu_bn_apply_jvp, "cgan_maxpool2_jvp": _emu_maxpool2_jvp,
-             "cgan_softmax_jvp": _emu_softmax_jvp, "cgan_metric_tensor_f64": _emu_metric_tensor_f64}
+_EMULATED = {name: getattr(EmulatedLib, name) for name in (
+    "cgan_act_jvp", "cgan_bn_apply_jvp", "cgan_maxpool2_jvp", "cgan_softmax_jvp", "cgan_metric_tensor_f64")}
 
 
 @pytest.fixture

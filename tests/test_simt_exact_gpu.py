@@ -44,7 +44,7 @@ import pytest
 import torch
 
 from compare_gan_b200 import _lib
-from tests.abi_emulator import emulated_library, rna_tf32
+from tests.abi_emulator import emulated_library, relu_gate, relu_mask, rna_tf32
 from tests.test_tc_exact_gpu import contract64, out_hw
 
 EXACT = 2 ** 24 - 1
@@ -414,7 +414,7 @@ def draw_conv(c, rng, random=False):
   if c.residual:
     ex["residual"] = side(shape)
   if c.leak is not None:
-    ex["mask"] = rng.standard_normal(shape).astype(np.float32)
+    ex["mask"] = relu_mask(rng, shape)
   return a, b, ex
 
 
@@ -433,8 +433,8 @@ def conv_expected(c, a, b, ex):
   if c.relu:
     y, y64 = np.maximum(y, np.float32(0)), np.maximum(y64, 0.0)
   if "mask" in ex:
-    y = np.where(ex["mask"] > 0, y, np.float32(c.leak) * y)
-    y64 = np.where(ex["mask"] > 0, y64, c.leak * y64)
+    y = relu_gate(ex["mask"], y, c.leak)
+    y64 = relu_gate(ex["mask"], y64, c.leak)
   if c.round_out:
     y = rna_tf32(y)
   return y, y64, scale

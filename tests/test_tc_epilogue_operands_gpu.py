@@ -16,7 +16,7 @@ import pytest
 import torch
 
 from compare_gan_b200 import _lib
-from tests.abi_emulator import rna_tf32
+from tests.abi_emulator import relu_gate, rna_tf32
 from tests.test_tc_exact_gpu import (K, NO_HALO, Case, assert_path, check, check_case, desc, dgrad, draw, fwd,  # noqa: F401
                                      mt2_batch, options, out_hw, reference, run, same_bits)
 
@@ -94,7 +94,7 @@ def algebra(c, y0, ex, round_out):
   if c.relu:
     y = np.maximum(y, f(0))
   if "mask" in ex:
-    y = np.where(ex["mask"] > 0, y, f(c.leak) * y)
+    y = relu_gate(ex["mask"], y, c.leak)
   return rna_tf32(y) if round_out else y
 
 

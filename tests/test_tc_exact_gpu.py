@@ -29,7 +29,7 @@ import torch
 import torch.nn.functional as F
 
 from compare_gan_b200 import _lib
-from tests.abi_emulator import emulated_library, rna_tf32
+from tests.abi_emulator import emulated_library, relu_gate, relu_mask, rna_tf32
 
 TAU = 1e-4
 WORST = {}          # path -> (worst err / A, case) of this session; printed when the module finishes
@@ -306,8 +306,9 @@ def seed_of(c, salt=0):
   return (sum(ord(ch) * (i + 1) for i, ch in enumerate(c.id)) + salt) % (2 ** 31)
 
 
-def draw(c, salt=0):
-  """Seeded TF32-exact operands a, b and the epilogue tensors of the case."""
+def draw(c, salt=0, mask_zeros=True):
+  """Seeded TF32-exact operands a, b and the epilogue tensors of the case.  The (leaky-)ReLU mask holds exact +-0 where
+  the two rules part ways; mask_zeros=False draws it as it was drawn before it had them (the same normal values)."""
   rng = np.random.RandomState(seed_of(c, salt))
   sa, sb = operand_shapes(c)
   a = rna_tf32(rng.standard_normal(sa).astype(np.float32))
@@ -320,7 +321,7 @@ def draw(c, salt=0):
   if c.residual:
     ex["residual"] = (4.0 * rng.standard_normal(shape)).astype(np.float32)
   if c.leak is not None:
-    ex["mask"] = rng.standard_normal(shape).astype(np.float32)
+    ex["mask"] = relu_mask(rng, shape) if mask_zeros else rng.standard_normal(shape).astype(np.float32)
   return a, b, ex
 
 
@@ -337,7 +338,7 @@ def reference(c, a, b, ex):
   if c.relu:
     y = np.maximum(y, 0.0)
   if "mask" in ex:
-    y = np.where(ex["mask"] > 0, y, c.leak * y)
+    y = relu_gate(ex["mask"], y, c.leak)
   return y, scale
 
 
@@ -570,7 +571,7 @@ def test_fused_epilogue_is_exact_fp32_algebra(K, c):
   shape = out_shape(c)
   bias = (4.0 * rng.standard_normal(shape[-1])).astype(np.float32)
   res = (4.0 * rng.standard_normal(shape)).astype(np.float32)
-  mask = rng.standard_normal(shape).astype(np.float32)
+  mask = relu_mask(rng, shape)
   f = np.float32
 
   def with_ep(round_out=False, **ep):
@@ -584,9 +585,9 @@ def test_fused_epilogue_is_exact_fp32_algebra(K, c):
   y0 = with_ep()
   yb = (y0 + bias).astype(f)
   assert same_bits(with_ep(bias=1), yb), "%s: + bias" % c.id
-  assert same_bits(with_ep(leak=0.2), np.where(mask > 0, y0, f(0.2) * y0)), "%s: mask without bias" % c.id
+  assert same_bits(with_ep(leak=0.2), relu_gate(mask, y0, 0.2)), "%s: mask without bias" % c.id
   for leak in (0.0, 0.2):
-    assert same_bits(with_ep(bias=1, leak=leak), np.where(mask > 0, yb, f(leak) * yb)), "%s: + bias, mask %g" % (c.id, leak)
+    assert same_bits(with_ep(bias=1, leak=leak), relu_gate(mask, yb, leak)), "%s: + bias, mask %g" % (c.id, leak)
   assert same_bits(with_ep(round_out=True, bias=1), rna_tf32(yb)), "%s: + bias, rounded" % c.id
   if c.op == "fwd":           # the forward entry takes the residual and the plain ReLU as well
     ybr = (yb + res).astype(f)

@@ -18,7 +18,7 @@ import torch
 
 from oracle import nets as onets
 from oracle import tf_ops as T
-from tests.abi_emulator import attention_tf32_model
+from tests.abi_emulator import attention_tf32_model, relu_pass
 from tests.gpu_util import ReluSigns, assert_close, compare_grads, make_inputs, make_pair, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -218,7 +218,7 @@ class _InSitu(object):
         if kw["bias"] is not None:
           ref = ref + t(kw["bias"])
         if kw.get("mask") is not None:
-          ref = torch.where(t(kw["mask"]) > 0, ref, float(kw["mask_leak"]) * ref)
+          ref = torch.where(relu_pass(t(kw["mask"]), kw["mask_leak"]), ref, float(kw["mask_leak"]) * ref)
         if kw["round_out"]:
           ref = T.rna_tf32(ref)
       else:
